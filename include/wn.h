@@ -26,7 +26,9 @@
 extern "C" {
 #endif
 
-#define WN_ABI_VERSION 2
+/* 3 = 2 plus streaming (wn_stream_*, wn_upsample_cone, wn_decode_stream); no struct of version 2 changed, and
+ * wn_create accepts a wn_config that says 2 */
+#define WN_ABI_VERSION 3
 
 typedef enum wn_status {
     WN_OK = 0,
@@ -151,7 +153,8 @@ typedef struct wn_plan_info {
 
 int32_t wn_abi_version(void);
 /* sizeof() of the structs of this header as the library was compiled, in the order wn_config, wn_weights,
- * wn_generate_args, wn_plan_info, wn_upsampler; n = capacity of `out`, the return value the number written.  Lets a binding
+ * wn_generate_args, wn_plan_info, wn_upsampler, wn_stream_open_args, wn_stream_chunk; n = capacity of `out`, the
+ * return value the number written.  Lets a binding
  * that transcribes the structs (ctypes, cgo, JNI) check its layout before the first real call. */
 int32_t wn_struct_sizes(int32_t* out, int32_t n);
 const char* wn_last_error(void);
@@ -201,6 +204,57 @@ int32_t wn_sync(void* handle);
 int32_t wn_generate_host(void* handle, const wn_generate_args* args);
 
 int32_t wn_get_plan(void* handle, int32_t batch, wn_plan_info* out);
+
+/* ---- Streaming (ABI 3): one utterance made in consecutive chunks, bit-identical to one wn_generate call over the
+ * whole utterance with the same weights, noise and conditioning, for any split.  What links step t to step t+1 --
+ * the older-tap history rings, the fed-back sample, the Philox step -- stays in a device buffer the stream owns.
+ * Engine 5 only, at most one batch tile (4 utterances), no teacher forcing.  Several streams may be open on one
+ * handle and called in turn; the handle still runs one call at a time, and wn_sync(handle) waits for a chunk. */
+typedef struct wn_stream_open_args {
+    int32_t B;                     /* utterances, 1..4                                                             */
+    const float* g;                /* DEVICE (B,gin) or NULL; read once, at open                                    */
+    const float* initial;          /* DEVICE, as wn_generate_args; copied at open                                   */
+    int32_t initial_index;
+    const int32_t* initial_rows;
+    const float* initial_dense;
+    uint32_t flags;                /* WN_FLAG_*                                                                     */
+    int32_t noise_kind;            /* WN_NOISE_*: PHILOX draws the noise of the absolute step; REPLAY takes each
+                                      chunk's (T,B,.) rows from the chunk's wn_generate_args                        */
+    uint64_t seed;
+    int32_t philox_row0;
+    void* stream;                  /* cudaStream_t of the open (it returns after the set-up is complete)            */
+    int32_t reserved[6];
+} wn_stream_open_args;
+
+/* Where a chunk's conditioning FRAMES (wn_generate_args.c_frames, n_frames of them) sit in the utterance. */
+typedef struct wn_stream_chunk {
+    int64_t frame_offset;          /* utterance frame index of c_frames[..., 0]                                      */
+    int64_t frames_total;          /* frames of the utterance received so far                                       */
+    int32_t final;                 /* 1: frames_total is the whole utterance; no chunk may follow this one          */
+    int32_t reserved[5];
+} wn_stream_chunk;
+
+int32_t wn_stream_open(void* handle, const wn_stream_open_args* args, void** stream);
+/* Generate the next chunk->T samples.  chunk: B as opened; T; c (B,T,C) sample-rate conditioning of these samples
+ * or c_frames + n_frames with `where`; replay noise (T,B,.); outputs and params_out (B,.,T) of this chunk;
+ * g, initial*, T_test and test_* unset.  `where` may be NULL without c_frames (then it can still mark the end).
+ * WN_ERR_STATE after wn_load_weights changed the handle's weights or after a final chunk. */
+int32_t wn_stream_generate(void* stream, const wn_generate_args* chunk, const wn_stream_chunk* where);
+/* Absolute step of the next sample (samples generated so far). */
+int64_t wn_stream_position(void* stream);
+int32_t wn_stream_close(void* stream);
+
+/* Device-less: the conditioning frames [*f_lo, *f_hi) that samples [t_lo, t_hi) of an utterance need, given n_frames
+ * received (final = 1: that is all of them), and *n_ready = how many samples from the start are known from those
+ * frames whatever follows (for final, the upsampled length).  Only scales, conv_in_ks and indent of `u` are read.  */
+int32_t wn_upsample_cone(const wn_upsampler* u, int64_t n_frames, int32_t final, int64_t t_lo, int64_t t_hi,
+                         int64_t* f_lo, int64_t* f_hi, int64_t* n_ready);
+
+/* wn_decode over one chunk of an utterance: `carry` (DEVICE, B floats, zero before the first chunk) holds the
+ * inv_preemphasis recursion between chunks; lengths are relative to the chunk. */
+int32_t wn_decode_stream(const float* y_scalar, const int32_t* y_index, int32_t B, int32_t T, const int32_t* lengths,
+                         int32_t input_type, int32_t quantize_channels, float preemphasis_coef, float global_gain_scale,
+                         float* out_float, int16_t* out_pcm16, float* carry, void* stream);
 
 /* Device-less planning + packing, for host-logic tests and tooling: computes the plan for
  * `cfg` assuming `num_sms` SMs / `smem_per_cta` bytes, and (if `packed` != NULL) writes the

@@ -18,7 +18,7 @@ SOURCES = [os.path.join(HERE, "csrc", "wn_host.cu")]
 HEADERS = [os.path.join(HERE, "csrc", f) for f in ("wn_plan.h", "wn_kernel.cuh", "wn7_plan.h", "wn7_kernel.cuh",
                                                      "wn7_host.cuh", "wn_aux.cuh")] + [os.path.join(ROOT, "include", "wn.h")]
 
-WN_ABI_VERSION = 2
+WN_ABI_VERSION = 3
 WN_INPUT_SCALAR, WN_INPUT_ONEHOT = 0, 1
 WN_HEAD_MOL, WN_HEAD_GAUSS, WN_HEAD_SOFTMAX = 0, 1, 2
 WN_NOISE_REPLAY, WN_NOISE_PHILOX = 0, 1
@@ -67,6 +67,17 @@ class wn_upsampler(C.Structure):
                 ("conv_in_w", _f32p), ("conv_in_ks", C.c_int32), ("indent", C.c_int32), ("reserved", C.c_int32 * 5)]
 
 
+class wn_stream_open_args(C.Structure):
+    _fields_ = [("B", C.c_int32), ("g", C.c_void_p), ("initial", C.c_void_p), ("initial_index", C.c_int32),
+                ("initial_rows", C.c_void_p), ("initial_dense", C.c_void_p), ("flags", C.c_uint32),
+                ("noise_kind", C.c_int32), ("seed", C.c_uint64), ("philox_row0", C.c_int32), ("stream", C.c_void_p),
+                ("reserved", C.c_int32 * 6)]
+
+
+class wn_stream_chunk(C.Structure):
+    _fields_ = [("frame_offset", C.c_int64), ("frames_total", C.c_int64), ("final", C.c_int32),
+                ("reserved", C.c_int32 * 5)]
+
 WN_DECODE_RAW, WN_DECODE_MULAW, WN_DECODE_MULAW_QUANTIZE = 0, 1, 2
 
 
@@ -82,6 +93,10 @@ class wn_plan_info(C.Structure):
 
     def as_dict(self):
         return {n: getattr(self, n) for n, _ in self._fields_ if n != "reserved"}
+
+
+# the structs in wn_struct_sizes order
+STRUCTS = (wn_config, wn_weights, wn_generate_args, wn_plan_info, wn_upsampler, wn_stream_open_args, wn_stream_chunk)
 
 
 class Wn7Pass(C.Structure):
@@ -130,7 +145,9 @@ def plan_passes(cfg, batch=1, num_sms=132, smem=232448):
 # every symbol include/wn.h declares (tests check the .so exports all of them)
 EXPORTS = ["wn_abi_version", "wn_struct_sizes", "wn_last_error", "wn_create", "wn_destroy", "wn_load_weights",
            "wn_generate", "wn_sync", "wn_generate_host", "wn_get_plan", "wn_plan_only",
-           "wn_pack_cta", "wn_plan_passes", "wn_load_upsampler", "wn_upsample", "wn_decode", "wn_sample_mol", "wn_sample_gauss"]
+           "wn_pack_cta", "wn_plan_passes", "wn_load_upsampler", "wn_upsample", "wn_decode", "wn_sample_mol", "wn_sample_gauss",
+           "wn_stream_open", "wn_stream_generate", "wn_stream_position", "wn_stream_close", "wn_upsample_cone",
+           "wn_decode_stream"]
 
 
 def nvcc_command(out=LIB_PATH):
@@ -209,19 +226,27 @@ def _bind(L):
     L.wn_sample_mol.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                 C.c_void_p, C.c_void_p]
     L.wn_sample_gauss.argtypes = L.wn_sample_mol.argtypes
+    L.wn_stream_open.argtypes = [C.c_void_p, C.POINTER(wn_stream_open_args), C.POINTER(C.c_void_p)]
+    L.wn_stream_generate.argtypes = [C.c_void_p, C.POINTER(wn_generate_args), C.POINTER(wn_stream_chunk)]
+    L.wn_stream_position.argtypes = [C.c_void_p]
+    L.wn_stream_close.argtypes = [C.c_void_p]
+    _i64p = C.POINTER(C.c_int64)
+    L.wn_upsample_cone.argtypes = [C.POINTER(wn_upsampler), C.c_int64, C.c_int32, C.c_int64, C.c_int64, _i64p, _i64p,
+                                   _i64p]
+    L.wn_decode_stream.argtypes = L.wn_decode.argtypes[:-1] + [C.c_void_p, C.c_void_p]
     for n in EXPORTS:
         if n == "wn_struct_sizes" and not hasattr(L, n):
             continue                       # an older build of the same ABI (A/B experiments through WN_LIB_PATH)
         fn = getattr(L, n)
         if n != "wn_last_error":
-            fn.restype = C.c_int32
+            fn.restype = C.c_int64 if n == "wn_stream_position" else C.c_int32
     if L.wn_abi_version() != WN_ABI_VERSION:
         raise RuntimeError("libwn.so ABI version mismatch")
-    sizes = (C.c_int32 * 5)()
+    sizes = (C.c_int32 * len(STRUCTS))()
     if hasattr(L, "wn_struct_sizes"):
         L.wn_struct_sizes.argtypes = [C.POINTER(C.c_int32), C.c_int32]
-    if hasattr(L, "wn_struct_sizes") and L.wn_struct_sizes(sizes, 5) == 5:
-        mine = [C.sizeof(t) for t in (wn_config, wn_weights, wn_generate_args, wn_plan_info, wn_upsampler)]
+    if hasattr(L, "wn_struct_sizes") and L.wn_struct_sizes(sizes, len(STRUCTS)) == len(STRUCTS):
+        mine = [C.sizeof(t) for t in STRUCTS]
         if list(sizes) != mine:
             raise RuntimeError("libwn.so struct layout mismatch: library %s, binding %s" % (list(sizes), mine))
     _lib = L

@@ -13,7 +13,7 @@ static int32_t build_plan7(const wn_config& c, int batch, int num_sms, long long
                            std::vector<Wn7Pass>& passes, std::vector<int>& ringtab) {
     memset(&pl, 0, sizeof(pl));
     passes.clear();
-    if (c.abi_version != WN_ABI_VERSION) return fail(WN_ERR_INVALID, "wn_config.abi_version mismatch");
+    if (c.abi_version != WN_ABI_VERSION && c.abi_version != 2) return fail(WN_ERR_INVALID, "wn_config.abi_version mismatch");
     if (c.layers < 1 || c.stacks < 1 || c.layers % c.stacks != 0)
         return fail(WN_ERR_INVALID, "layers must be a positive multiple of stacks (wavenet.py:117)");
     if (c.gate_channels < 2 || (c.gate_channels & 1)) return fail(WN_ERR_INVALID, "gate_channels must be even");

@@ -12,6 +12,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <math.h>
+#include <algorithm>
 
 namespace wnaux {
 
@@ -54,20 +55,24 @@ __global__ void frames_to_fc_kernel(const float* __restrict__ c, float* __restri
 // global memory in (B,T,C) layout.
 //   level j:  a_j[u] = sum_{k=0}^{2s} w_j[k] * st[u + k - s],   st[v] = a_{j-1}[min(floor(v * rscale), n_{j-1}-1)] for
 //   0 <= v < n_j, 0 outside (Conv2d padding (0, s), upsample.py:41-43; Stretch2d upsample.py:19-21)
+// Windows (streaming): `h` holds rows [f_off, f_off+Fw) of level 0, whose full length is n0 (WNAUX_UNBOUNDED while more
+// frames may follow), and output sample i is sample t_off + i of the whole utterance.  Every index, the zero padding
+// and the clamp are those of the whole sequence, so a window equals the same samples of a one-shot upsample.
+#define WNAUX_UNBOUNDED (1 << 30)
 template <int TS>
-__global__ void upsample_kernel(const float* __restrict__ h /* (B,F0,C) */, const float* __restrict__ filters,
-                                const __grid_constant__ UpsampleDesc d,
-                                int C, int F0, int T_out, float* __restrict__ out /* (B,T_out,C) */) {
+__global__ void upsample_kernel(const float* __restrict__ h /* (B,Fw,C) */, const float* __restrict__ filters,
+                                const __grid_constant__ UpsampleDesc d, int C, int Fw, int f_off, int n0, int t_off,
+                                int T_out, float* __restrict__ out /* (B,T_out,C) */) {
     extern __shared__ float sm[];
     const int b = blockIdx.y, t0 = blockIdx.x * TS;
     const int J = d.n_scales;
     // length of every level and the index range this tile needs from it (block-uniform: one thread fills the table)
     __shared__ int n[WNAUX_MAX_SCALES + 1], lo[WNAUX_MAX_SCALES + 1], hi[WNAUX_MAX_SCALES + 1];
     if (threadIdx.x == 0) {
-        n[0] = F0;
-        for (int j = 1; j <= J; ++j) n[j] = n[j - 1] * d.scales[j - 1];
-        lo[J] = t0 + d.indent;
-        hi[J] = min(t0 + TS, T_out) - 1 + d.indent;
+        n[0] = n0;
+        for (int j = 1; j <= J; ++j) n[j] = n0 >= WNAUX_UNBOUNDED ? WNAUX_UNBOUNDED : n[j - 1] * d.scales[j - 1];
+        lo[J] = t_off + t0 + d.indent;
+        hi[J] = t_off + min(t0 + TS, T_out) - 1 + d.indent;
         for (int j = J; j >= 1; --j) {
             const int s = d.scales[j - 1];
             const int vlo = max(lo[j] - s, 0), vhi = min(hi[j] + s, n[j] - 1);
@@ -82,7 +87,7 @@ __global__ void upsample_kernel(const float* __restrict__ h /* (B,F0,C) */, cons
     {
         const int len = hi[0] - lo[0] + 1;
         for (int i = threadIdx.x; i < len * C; i += blockDim.x)
-            cur[i] = h[((size_t)b * F0 + lo[0]) * C + i];
+            cur[i] = h[((size_t)b * Fw + (lo[0] - f_off)) * C + i];
     }
     __syncthreads();
     for (int j = 1; j <= J; ++j) {
@@ -101,12 +106,40 @@ __global__ void upsample_kernel(const float* __restrict__ h /* (B,F0,C) */, cons
                     a = fmaf(w[k], cur[(size_t)(src - lo[j - 1]) * C + ch], a);
                 }
             }
-            if (last) out[((size_t)b * T_out + (u - d.indent)) * C + ch] = a;
+            if (last) out[((size_t)b * T_out + (u - d.indent - t_off)) * C + ch] = a;
             else nxt[i] = a;
         }
         __syncthreads();
         float* t = cur; cur = nxt; nxt = t;
     }
+}
+
+// Host mirror of the table upsample_kernel builds: rows [*r_lo, *r_hi] of level 0 that output samples [t_lo, t_hi)
+// read when level 0 has n0 rows (WNAUX_UNBOUNDED: no right edge).  *inside: no index of that cone reaches past the
+// first n_in rows of level 0 at any level (neither the zero padding nor the clamp of a sequence that ends there), so
+// the samples are the same for every sequence that starts with those n_in rows.
+inline void cone_rows(const UpsampleDesc& d, int n0, int n_in, int t_lo, int t_hi, int* r_lo, int* r_hi, bool* inside) {
+    const int J = d.n_scales;
+    int n[WNAUX_MAX_SCALES + 1], m[WNAUX_MAX_SCALES + 1];
+    n[0] = n0;
+    m[0] = n_in;
+    for (int j = 1; j <= J; ++j) {
+        n[j] = n0 >= WNAUX_UNBOUNDED ? WNAUX_UNBOUNDED : n[j - 1] * d.scales[j - 1];
+        m[j] = m[j - 1] * d.scales[j - 1];
+    }
+    int lo = t_lo + d.indent, hi = t_hi - 1 + d.indent;
+    bool ok = hi < m[J];
+    for (int j = J; j >= 1; --j) {
+        const int s = d.scales[j - 1];
+        const int vlo = std::max(lo - s, 0), vhi = std::min(hi + s, n[j] - 1);
+        ok = ok && hi + s < m[j];
+        lo = std::min((int)floorf((float)vlo * d.rscale[j - 1]), n[j - 1] - 1);
+        hi = std::min((int)floorf((float)vhi * d.rscale[j - 1]), n[j - 1] - 1);
+        ok = ok && (int)floorf((float)vhi * d.rscale[j - 1]) < m[j - 1];
+    }
+    *r_lo = lo;
+    *r_hi = hi;
+    *inside = ok;
 }
 
 // ---- decode -------------------------------------------------------------------------------------------------
@@ -115,15 +148,17 @@ enum { DEC_RAW = 0, DEC_MULAW = 1, DEC_MULAW_QUANTIZE = 2 };
 // One block per utterance; chunks of CH samples: pointwise inverse companding by all threads, the one-pole
 // recursion by thread 0 (y[n] = x[n] + coef*y[n-1], each operation rounded to float32 exactly like
 // scipy.signal.lfilter's float32 loop), then gain / clip / int16 by all threads.
+// `carry` (B, or NULL for a zero start): coef * y[-1] on entry, coef * y[T-1] on exit, so that consecutive chunks of an
+// utterance decode to the bits one call over the whole utterance gives.
 template <int CH>
 __global__ void decode_kernel(const float* __restrict__ y_scalar, const int* __restrict__ y_index, int T, const int* __restrict__ lengths,
                               int kind, float mu, float coef, float gain, float* __restrict__ out_float,
-                              short* __restrict__ out_pcm) {
+                              short* __restrict__ out_pcm, float* __restrict__ carry = nullptr) {
     __shared__ float chunk[CH];
     __shared__ float carry_s;
     const int b = blockIdx.x;
     const int len = lengths ? min(lengths[b], T) : T;
-    if (threadIdx.x == 0) carry_s = 0.f;
+    if (threadIdx.x == 0) carry_s = carry ? carry[b] : 0.f;
     __syncthreads();
     for (int base = 0; base < T; base += CH) {
         const int nthis = min(CH, T - base);
@@ -166,6 +201,7 @@ __global__ void decode_kernel(const float* __restrict__ y_scalar, const int* __r
         }
         __syncthreads();
     }
+    if (carry && threadIdx.x == 0) carry[b] = carry_s;
 }
 
 }  // namespace wnaux

@@ -57,7 +57,8 @@ static int align_up(long long v, int a) { return (int)(((v + a - 1) / a) * a); }
 static int32_t build_plan(const wn_config& c, int batch, int num_sms, long long smem_cap, WnPlan& pl,
                           std::vector<int>& ringtab) {
     memset(&pl, 0, sizeof(pl));
-    if (c.abi_version != WN_ABI_VERSION) return fail(WN_ERR_INVALID, "wn_config.abi_version mismatch");
+    // version 3 only added entry points: a version-2 caller's structs are the same
+    if (c.abi_version != WN_ABI_VERSION && c.abi_version != 2) return fail(WN_ERR_INVALID, "wn_config.abi_version mismatch");
     if (c.layers < 1 || c.stacks < 1 || c.layers % c.stacks != 0)
         return fail(WN_ERR_INVALID, "layers must be a positive multiple of stacks (wavenet.py:117)");
     if (c.gate_channels < 2 || (c.gate_channels & 1)) return fail(WN_ERR_INVALID, "gate_channels must be even");
@@ -453,6 +454,7 @@ struct WnHandle {
     int num_sms = 0;
     long long smem_cap = 0;
     bool have_weights = false;
+    uint64_t weight_gen = 0;      // bumped by every weight / upsampler upload: an open stream made with older ones stops
     WnPlan base;                  // plan for BT=1 (partition + blob layout are batch independent)
     std::vector<int> ringtab;
     float *d_wpack = nullptr, *d_cwpack = nullptr, *d_wg = nullptr, *d_first_w = nullptr, *d_first_b = nullptr;
@@ -466,7 +468,7 @@ struct WnHandle {
     cudaStream_t last_stream = nullptr;
     bool pending = false;
     int64_t launches = 0;
-    bool attr_set[20] = {};
+    bool attr_set[40] = {};       // [20, 40): the stream instantiations
     size_t l2_persist_bytes = 0, l2_window_max = 0;   // persisting-L2 carve-out
     int l2_mode = 0;                                  // WN_L2_PERSIST: 1 = packed weights, 2 = exchange buffer
     size_t wpack_bytes = 0;
@@ -486,7 +488,16 @@ static int32_t ensure(T** ptr, size_t* have, size_t need) {
 static int max_tile(int engine) { return std::max(1, std::min(8, env_int("WN_MAX_TILE", engine == 7 ? 8 : 4))); }
 static int bt_index(int BT) { return BT == 1 ? 0 : BT == 2 ? 1 : BT == 4 ? 2 : 3; }
 
-static int32_t launch_chunk(WnHandle* h, const wn_generate_args* a, int b0, int Bc, cudaStream_t st) {
+// One launch of a stream (wn_stream_generate): the stream's state buffer and where the launch starts.
+struct StreamCtx {
+    float* state;          // rings then feedback (wn_kernel.cuh WnPtrs::state); rings in global memory live in it
+    int state_load;        // 0 for the first chunk: zero history, feedback from initial*
+    unsigned t_base;       // absolute step of the chunk's first sample
+    const float* gbias;    // Wg . g, computed at open (NULL without global conditioning)
+};
+
+static int32_t launch_chunk(WnHandle* h, const wn_generate_args* a, int b0, int Bc, cudaStream_t st,
+                            const StreamCtx* sc = nullptr) {
     WnPlan pl;
     std::vector<int> rt;
     int32_t rc = build_plan(h->cfg, Bc, h->num_sms, h->smem_cap, pl, rt);
@@ -501,7 +512,7 @@ static int32_t launch_chunk(WnHandle* h, const wn_generate_args* a, int b0, int 
     rc = ensure(&h->d_xbuf, &h->xbuf_bytes, xb);
     if (rc) return rc;
     CUDA_TRY(cudaMemsetAsync(h->d_xbuf, 0, xb, st));
-    if (!pl.ring_in_smem) {
+    if (!pl.ring_in_smem && !sc) {         // a stream's global-memory rings are its state buffer (zeroed at open)
         const size_t rb = std::max<size_t>(16, (size_t)pl.P * pl.ring_pos_total * pl.RA4 * BT * sizeof(float));
         rc = ensure(&h->d_ring, &h->ring_bytes, rb);
         if (rc) return rc;
@@ -509,7 +520,12 @@ static int32_t launch_chunk(WnHandle* h, const wn_generate_args* a, int b0, int 
     }
     WnPtrs pp;
     memset(&pp, 0, sizeof(pp));
-    if (c.gin_channels > 0) {
+    if (sc) {
+        pp.state = sc->state;
+        pp.state_load = sc->state_load;
+        pp.t_base = sc->t_base;
+        pp.gbias = sc->gbias;
+    } else if (c.gin_channels > 0) {
         if (!a->g) return fail(WN_ERR_INVALID, "g is required (gin_channels > 0), cf. train.py:72-80 sanity_check");
         const size_t gb = (size_t)Bc * pl.L * pl.G * sizeof(float);
         rc = ensure(&h->d_gbias, &h->gbias_bytes, gb);
@@ -526,7 +542,7 @@ static int32_t launch_chunk(WnHandle* h, const wn_generate_args* a, int b0, int 
     pp.first_w = h->d_first_w;
     pp.first_b = h->d_first_b;
     pp.xbuf = h->d_xbuf;
-    pp.ring_g = h->d_ring;
+    pp.ring_g = (sc && !pl.ring_in_smem) ? sc->state : h->d_ring;
     pp.ringtab = h->d_ringtab;
     pp.err = h->d_err;
     pp.c = a->c ? a->c + (size_t)b0 * T * pl.C : nullptr;
@@ -586,22 +602,26 @@ static int32_t launch_chunk(WnHandle* h, const wn_generate_args* a, int b0, int 
                    env_int("WN_LEAN", 0) != 0) ? 1 : 0;
     }
     const void* fn = nullptr;
-#define WN_PICK(BT_)                                                                          \
-    fn = var == 0 ? (const void*)wn::wn_persistent_kernel<BT_, 1, 1>                          \
-       : var == 1 ? (const void*)wn::wn_persistent_kernel<BT_, 2, 2>                          \
-       : var == 2 ? (const void*)wn::wn_persistent_kernel<BT_, 4, 2>                          \
-                  : (const void*)wn::wn_persistent_kernel<BT_, 8, 8>
+    // stream launches take the STREAM instantiations (wn_kernel.cuh Engine); a stream holds at most one tile of 4
+#define WN_PICK(BT_, S_)                                                                      \
+    fn = var == 0 ? (const void*)wn::wn_persistent_kernel<BT_, 1, 1, false, S_>               \
+       : var == 1 ? (const void*)wn::wn_persistent_kernel<BT_, 2, 2, false, S_>               \
+       : var == 2 ? (const void*)wn::wn_persistent_kernel<BT_, 4, 2, false, S_>               \
+                  : (const void*)wn::wn_persistent_kernel<BT_, 8, 8, false, S_>
+    if (sc && BT > 4) return fail(WN_ERR_INVALID, "a stream holds at most 4 utterances");
     switch (BT) {
-        case 1: WN_PICK(1); break;
-        case 2: WN_PICK(2); break;
-        case 4: WN_PICK(4); break;
-        default: WN_PICK(8); break;
+        case 1: if (sc) WN_PICK(1, true); else WN_PICK(1, false); break;
+        case 2: if (sc) WN_PICK(2, true); else WN_PICK(2, false); break;
+        case 4: if (sc) WN_PICK(4, true); else WN_PICK(4, false); break;
+        default: WN_PICK(8, false); break;
     }
 #undef WN_PICK
     if (pl.lean)      // the lean kernels: same plan, same packed weights, the lean stage path instead of the generic one
-        fn = var == 1 ? (const void*)wn::wn_persistent_kernel<1, 2, 2, true>
-                      : (const void*)wn::wn_persistent_kernel<1, 4, 2, true>;
-    const int ai = pl.lean ? 16 + var : bt_index(BT) * 4 + var;
+        fn = sc ? (var == 1 ? (const void*)wn::wn_persistent_kernel<1, 2, 2, true, true>
+                            : (const void*)wn::wn_persistent_kernel<1, 4, 2, true, true>)
+                : (var == 1 ? (const void*)wn::wn_persistent_kernel<1, 2, 2, true>
+                            : (const void*)wn::wn_persistent_kernel<1, 4, 2, true>);
+    const int ai = (pl.lean ? 16 + var : bt_index(BT) * 4 + var) + (sc ? 20 : 0);
     if (!h->attr_set[ai]) {
         CUDA_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_cap));
         h->attr_set[ai] = true;
@@ -686,9 +706,13 @@ static void fill_info7(const wn_config& c, const Wn7Plan& pl, wn_plan_info* out)
     out->streamed_bytes_per_step = streamed * pl.P;
 }
 
-static int32_t run_upsampler(WnHandle* h, const float* c_frames, int B, int F, int T, cudaStream_t st) {
+// c_frames (B,C,F) -> h->d_cup (B,T,C).  A stream passes a window: c_frames starts at utterance frame f_off, level 0
+// of the utterance has n0 rows (WNAUX_UNBOUNDED until the last frame is known) and the output starts at sample t_off.
+static int32_t run_upsampler(WnHandle* h, const float* c_frames, int B, int F, int T, cudaStream_t st, int f_off = 0,
+                             int n0 = -1, int t_off = 0) {
     const int C = h->ups_C;
     const int Fo = F - (h->ups_ks > 0 ? h->ups_ks - 1 : 0);
+    if (n0 < 0) n0 = Fo;
     int32_t rc = ensure(&h->d_hfr, &h->hfr_bytes, (size_t)B * Fo * C * sizeof(float));
     if (rc) return rc;
     rc = ensure(&h->d_cup, &h->cup_bytes, (size_t)B * T * C * sizeof(float));
@@ -706,8 +730,8 @@ static int32_t run_upsampler(WnHandle* h, const float* c_frames, int B, int F, i
         CUDA_TRY(cudaFuncSetAttribute(wnaux::upsample_kernel<TS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         h->ups_attr = true;
     }
-    wnaux::upsample_kernel<TS><<<dim3((T + TS - 1) / TS, B), 256, smem, st>>>(h->d_hfr, h->d_ups_filters, h->ups, C, Fo, T,
-                                                                            h->d_cup);
+    wnaux::upsample_kernel<TS><<<dim3((T + TS - 1) / TS, B), 256, smem, st>>>(h->d_hfr, h->d_ups_filters, h->ups, C, Fo,
+                                                                            f_off, n0, t_off, T, h->d_cup);
     CUDA_TRY(cudaGetLastError());
     h->launches += 2;
     return WN_OK;
@@ -858,10 +882,11 @@ extern "C" {
 
 int32_t wn_abi_version(void) { return WN_ABI_VERSION; }
 int32_t wn_struct_sizes(int32_t* out, int32_t n) {
-    const int32_t v[5] = {(int32_t)sizeof(wn_config), (int32_t)sizeof(wn_weights), (int32_t)sizeof(wn_generate_args),
-                          (int32_t)sizeof(wn_plan_info), (int32_t)sizeof(wn_upsampler)};
+    const int32_t v[7] = {(int32_t)sizeof(wn_config), (int32_t)sizeof(wn_weights), (int32_t)sizeof(wn_generate_args),
+                          (int32_t)sizeof(wn_plan_info), (int32_t)sizeof(wn_upsampler),
+                          (int32_t)sizeof(wn_stream_open_args), (int32_t)sizeof(wn_stream_chunk)};
     int32_t k = 0;
-    for (; k < 5 && k < n; ++k) out[k] = v[k];
+    for (; k < 7 && k < n; ++k) out[k] = v[k];
     return k;
 }
 const char* wn_last_error(void) { return g_err.c_str(); }
@@ -1029,8 +1054,9 @@ int32_t wn_load_weights(void* handle, const wn_weights* w) {
     int32_t rc = check_weights(h->cfg, w);
     if (rc) return rc;
     DeviceGuard guard(h->cfg.device);
+    h->weight_gen++;
     const wn_config& c = h->cfg;
-    auto upload = [&](float** dst, const std::vector<float>& src) -> int32_t {
+    auto upload =[&](float** dst, const std::vector<float>& src) -> int32_t {
         if (*dst) cudaFree(*dst);
         *dst = nullptr;
         CUDA_TRY(cudaMalloc((void**)dst, std::max<size_t>(16, src.size() * sizeof(float))));
@@ -1101,7 +1127,8 @@ int32_t wn_load_weights(void* handle, const wn_weights* w) {
     return WN_OK;
 }
 
-static int32_t validate_args(const WnHandle* h, const wn_generate_args* a) {
+// window_frames: c_frames is a window of the utterance (a stream chunk, checked by the caller), not all of it
+static int32_t validate_args(const WnHandle* h, const wn_generate_args* a, bool window_frames = false) {
     const wn_config& c = h->cfg;
     if (!a) return fail(WN_ERR_INVALID, "null args");
     if (a->B < 1 || a->T < 1) return fail(WN_ERR_INVALID, "B and T must be >= 1");
@@ -1109,7 +1136,9 @@ static int32_t validate_args(const WnHandle* h, const wn_generate_args* a) {
     if (a->c && a->c_frames) return fail(WN_ERR_INVALID, "give either c (sample rate) or c_frames, not both");
     if (c.cin_channels > 0 && !a->c && !a->c_frames) return fail(WN_ERR_INVALID, "c is required (cin_channels > 0), cf. train.py:82-87");
     if (c.cin_channels == 0 && (a->c || a->c_frames)) return fail(WN_ERR_INVALID, "c given but the model has no local conditioning");
-    if (a->c_frames) {
+    if (a->c_frames && window_frames) {
+        if (!h->have_ups) return fail(WN_ERR_STATE, "c_frames given but no upsampler was loaded (wn_load_upsampler)");
+    } else if (a->c_frames) {
         if (!h->have_ups) return fail(WN_ERR_STATE, "c_frames given but no upsampler was loaded (wn_load_upsampler)");
         const long long Fo = (long long)a->n_frames - (h->ups_ks > 0 ? h->ups_ks - 1 : 0);
         if (Fo < 1 || Fo * h->ups_total - 2LL * h->ups.indent != (long long)a->T)
@@ -1299,31 +1328,96 @@ int32_t wn_generate_host(void* handle, const wn_generate_args* a) {
     return wn_sync(handle);
 }
 
+// the geometry of an upsampler (everything but its weights); *filter_floats = taps of all smoothing filters
+static int32_t ups_desc(const wn_upsampler* u, wnaux::UpsampleDesc& d, long long& total, int& filter_floats) {
+    if (u->n_scales < 1 || u->n_scales > WNAUX_MAX_SCALES || !u->scales)
+        return fail(WN_ERR_INVALID, "upsampler needs 1..8 scales and their filters");
+    if (u->conv_in_ks < 0 || u->indent < 0) return fail(WN_ERR_INVALID, "bad conv_in / indent");
+    memset(&d, 0, sizeof(d));
+    d.n_scales = u->n_scales;
+    d.indent = u->indent;
+    int off = 0;
+    total = 1;
+    for (int j = 0; j < u->n_scales; ++j) {
+        const int s = u->scales[j];
+        if (s < 2 || s > 4096) return fail(WN_ERR_INVALID, "every upsample scale must be in [2,4096]");
+        d.scales[j] = s;
+        d.foff[j] = off;
+        d.rscale[j] = (float)(1.0 / (double)s);
+        off += 2 * s + 1;
+        total *= s;
+        if (total > (1 << 24)) return fail(WN_ERR_INVALID, "total upsample scale too large");
+    }
+    filter_floats = off;
+    return WN_OK;
+}
+
+// Frames [*f_lo, *f_hi) that samples [t_lo, t_hi) need and the samples known from the start (*n_ready), given
+// n_frames received (final: all of them).  Mirrors upsample_kernel's index table (wnaux::cone_rows).
+static int32_t ups_cone(const wnaux::UpsampleDesc& d, long long total, int ks, long long n_frames, bool final,
+                        long long t_lo, long long t_hi, long long* f_lo, long long* f_hi, long long* n_ready) {
+    const int lost = ks > 0 ? ks - 1 : 0;
+    const long long Fo = n_frames - lost;                 // rows of level 0 (conv_in outputs) known
+    *f_lo = *f_hi = 0;
+    *n_ready = 0;
+    if (t_lo < 0 || t_hi < t_lo) return fail(WN_ERR_INVALID, "bad sample range");
+    if (Fo < 1) return t_hi > t_lo ? fail(WN_ERR_INVALID, "no sample is known before conv_in has its first window") : WN_OK;
+    if (Fo * total >= WNAUX_UNBOUNDED) return fail(WN_ERR_INVALID, "utterance too long for the upsampler's 32-bit indices");
+    const int n0 = final ? (int)Fo : WNAUX_UNBOUNDED;
+    const long long full = std::max(0LL, Fo * total - 2LL * d.indent);   // the length if the utterance ended here
+    int lo, hi;
+    bool inside;
+    if (final) {
+        *n_ready = full;
+    } else {
+        // the cone grows with t, so the known samples are a prefix: bisect for its length
+        long long a = 0, b = full;
+        while (a < b) {
+            const long long m = (a + b + 1) / 2;
+            wnaux::cone_rows(d, n0, (int)Fo, (int)(m - 1), (int)m, &lo, &hi, &inside);
+            if (inside) a = m; else b = m - 1;
+        }
+        *n_ready = a;
+    }
+    if (t_hi > t_lo) {
+        if (t_hi > full) return fail(WN_ERR_INVALID, "sample range beyond the upsampled length of the frames");
+        wnaux::cone_rows(d, n0, (int)Fo, (int)t_lo, (int)t_hi, &lo, &hi, &inside);
+        *f_lo = lo;
+        *f_hi = (long long)hi + lost + 1;
+    }
+    return WN_OK;
+}
+
+int32_t wn_upsample_cone(const wn_upsampler* u, int64_t n_frames, int32_t final, int64_t t_lo, int64_t t_hi,
+                         int64_t* f_lo, int64_t* f_hi, int64_t* n_ready) {
+    if (!u || !f_lo || !f_hi || !n_ready) return fail(WN_ERR_INVALID, "null argument");
+    wnaux::UpsampleDesc d;
+    long long total, a, b, r;
+    int nf;
+    int32_t rc = ups_desc(u, d, total, nf);
+    if (rc) return rc;
+    rc = ups_cone(d, total, u->conv_in_ks, n_frames, final != 0, t_lo, t_hi, &a, &b, &r);
+    *f_lo = a;
+    *f_hi = b;
+    *n_ready = r;
+    return rc;
+}
+
 int32_t wn_load_upsampler(void* handle, const wn_upsampler* u) {
     WnHandle* h = (WnHandle*)handle;
     if (!h) return fail(WN_ERR_INVALID, "null handle");
     DeviceGuard guard(h->cfg.device);
     h->have_ups = false;
+    h->weight_gen++;
     if (!u) return WN_OK;
     if (u->channels != h->cfg.cin_channels || u->channels < 1) return fail(WN_ERR_INVALID, "upsampler channels != cin_channels");
     if (u->n_scales < 1 || u->n_scales > WNAUX_MAX_SCALES || !u->scales || !u->filters)
         return fail(WN_ERR_INVALID, "upsampler needs 1..8 scales and their filters");
     if ((u->conv_in_w != nullptr) != (u->conv_in_ks > 0) || u->indent < 0) return fail(WN_ERR_INVALID, "bad conv_in / indent");
-    memset(&h->ups, 0, sizeof(h->ups));
-    h->ups.n_scales = u->n_scales;
-    h->ups.indent = u->indent;
-    int off = 0;
     long long total = 1;
-    for (int j = 0; j < u->n_scales; ++j) {
-        const int s = u->scales[j];
-        if (s < 2 || s > 4096) return fail(WN_ERR_INVALID, "every upsample scale must be in [2,4096]");
-        h->ups.scales[j] = s;
-        h->ups.foff[j] = off;
-        h->ups.rscale[j] = (float)(1.0 / (double)s);
-        off += 2 * s + 1;
-        total *= s;
-        if (total > (1 << 24)) return fail(WN_ERR_INVALID, "total upsample scale too large");
-    }
+    int off = 0;
+    int32_t rc = ups_desc(u, h->ups, total, off);
+    if (rc) return rc;
     h->ups_total = (int)total;
     h->ups_C = u->channels;
     h->ups_ks = u->conv_in_ks;
@@ -1357,9 +1451,9 @@ int32_t wn_upsample(void* handle, const float* c_frames, int32_t B, int32_t n_fr
     return WN_OK;
 }
 
-int32_t wn_decode(const float* y_scalar, const int32_t* y_index, int32_t B, int32_t T, const int32_t* lengths,
-                  int32_t input_type, int32_t quantize_channels, float preemphasis_coef, float global_gain_scale,
-                  float* out_float, int16_t* out_pcm16, void* stream) {
+int32_t wn_decode_stream(const float* y_scalar, const int32_t* y_index, int32_t B, int32_t T, const int32_t* lengths,
+                         int32_t input_type, int32_t quantize_channels, float preemphasis_coef, float global_gain_scale,
+                         float* out_float, int16_t* out_pcm16, float* carry, void* stream) {
     if (B < 1 || T < 1) return fail(WN_ERR_INVALID, "B and T must be >= 1");
     if (!out_float && !out_pcm16) return fail(WN_ERR_INVALID, "no output buffer");
     if (input_type == WN_DECODE_MULAW_QUANTIZE ? !y_index : !y_scalar) return fail(WN_ERR_INVALID, "missing input for this input_type");
@@ -1367,8 +1461,177 @@ int32_t wn_decode(const float* y_scalar, const int32_t* y_index, int32_t B, int3
     if (input_type != WN_DECODE_RAW && quantize_channels < 2) return fail(WN_ERR_INVALID, "quantize_channels must be >= 2");
     wnaux::decode_kernel<1024><<<B, 256, 0, (cudaStream_t)stream>>>(y_scalar, y_index, T, lengths, input_type,
                                                                     (float)(quantize_channels - 1), preemphasis_coef,
-                                                                    global_gain_scale, out_float, (short*)out_pcm16);
+                                                                    global_gain_scale, out_float, (short*)out_pcm16, carry);
     CUDA_TRY(cudaGetLastError());
+    return WN_OK;
+}
+
+int32_t wn_decode(const float* y_scalar, const int32_t* y_index, int32_t B, int32_t T, const int32_t* lengths,
+                  int32_t input_type, int32_t quantize_channels, float preemphasis_coef, float global_gain_scale,
+                  float* out_float, int16_t* out_pcm16, void* stream) {
+    return wn_decode_stream(y_scalar, y_index, B, T, lengths, input_type, quantize_channels, preemphasis_coef,
+                            global_gain_scale, out_float, out_pcm16, nullptr, stream);
+}
+
+// ------------------------------------------------------------------------------------------
+// streams
+// ------------------------------------------------------------------------------------------
+struct WnStream {
+    WnHandle* h = nullptr;
+    int B = 0;
+    uint64_t weight_gen = 0;       // the handle's weights this stream was opened with
+    wn_stream_open_args open;      // initial* point into d_init (copies made at open)
+    float* d_state = nullptr;      // P x rings, then the feedback (wn_kernel.cuh WnPtrs::state)
+    float* d_gbias = nullptr;
+    float* d_init = nullptr;
+    long long t = 0;               // absolute step of the next sample
+    bool final = false;
+};
+
+int32_t wn_stream_open(void* handle, const wn_stream_open_args* a, void** stream) {
+    WnHandle* h = (WnHandle*)handle;
+    if (!h || !a || !stream) return fail(WN_ERR_INVALID, "null argument");
+    *stream = nullptr;
+    if (!h->have_weights) return fail(WN_ERR_STATE, "wn_stream_open before wn_load_weights");
+    if (h->engine != 5) return fail(WN_ERR_INVALID, "streaming runs on engine 5 only (WN_ENGINE=7 was chosen)");
+    const int tile = std::min(4, max_tile(5));
+    if (a->B < 1 || a->B > tile)
+        return fail(WN_ERR_INVALID, "a stream holds 1.." + std::to_string(tile) + " utterances (one batch tile)");
+    const wn_config& c = h->cfg;
+    if (c.gin_channels > 0 && !a->g) return fail(WN_ERR_INVALID, "g is required (gin_channels > 0), cf. train.py:72-80 sanity_check");
+    if (c.gin_channels == 0 && a->g) return fail(WN_ERR_INVALID, "g given but the model has no global conditioning");
+    if (a->noise_kind != WN_NOISE_REPLAY && a->noise_kind != WN_NOISE_PHILOX) return fail(WN_ERR_INVALID, "bad noise_kind");
+    DeviceGuard guard(c.device);
+    WnPlan pl;
+    std::vector<int> rt;
+    int32_t rc = build_plan(c, a->B, h->num_sms, h->smem_cap, pl, rt);
+    if (rc) return rc;
+    cudaStream_t st = (cudaStream_t)a->stream;
+    WnStream* s = new WnStream();
+    s->h = h;
+    s->B = a->B;
+    s->weight_gen = h->weight_gen;
+    s->open = *a;
+    auto bail = [&](int32_t code) {
+        cudaFree(s->d_state); cudaFree(s->d_gbias); cudaFree(s->d_init);
+        delete s;
+        return code;
+    };
+    const size_t state_floats = (size_t)pl.P * wn_state_ring_floats(pl) + wn_state_feedback_floats(pl);
+    if (cudaMalloc((void**)&s->d_state, state_floats * sizeof(float)) != cudaSuccess ||
+        cudaMalloc((void**)&s->d_init, ((size_t)2 + pl.O) * a->B * sizeof(float)) != cudaSuccess)
+        return bail(fail(WN_ERR_NOMEM, "cudaMalloc of the stream state failed"));
+    if (cudaMemsetAsync(s->d_state, 0, state_floats * sizeof(float), st) != cudaSuccess)
+        return bail(fail(WN_ERR_CUDA, "cudaMemsetAsync of the stream state failed"));
+    // the step-0 inputs are copied: the caller's buffers may go once open returns
+    float* init = s->d_init;
+    int32_t* init_rows = (int32_t*)(s->d_init + a->B);
+    float* init_dense = s->d_init + 2 * a->B;
+    auto copy = [&](void* dst, const void* src, size_t bytes) {
+        return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, st) == cudaSuccess;
+    };
+    if ((a->initial && !copy(init, a->initial, a->B * sizeof(float))) ||
+        (a->initial_rows && !copy(init_rows, a->initial_rows, a->B * sizeof(int32_t))) ||
+        (a->initial_dense && !copy(init_dense, a->initial_dense, (size_t)a->B * pl.O * sizeof(float))))
+        return bail(fail(WN_ERR_CUDA, "copying the initial input failed"));
+    s->open.initial = a->initial ? init : nullptr;
+    s->open.initial_rows = a->initial_rows ? init_rows : nullptr;
+    s->open.initial_dense = a->initial_dense ? init_dense : nullptr;
+    s->open.g = nullptr;
+    if (c.gin_channels > 0) {
+        // Wg . g once per stream (modules.py:148-152 recomputes it every step although g is constant)
+        if (cudaMalloc((void**)&s->d_gbias, (size_t)a->B * pl.L * pl.G * sizeof(float)) != cudaSuccess)
+            return bail(fail(WN_ERR_NOMEM, "cudaMalloc of the stream's global-conditioning bias failed"));
+        wn::wn_gbias_kernel<<<dim3(pl.L, a->B), 128, 0, st>>>(h->d_wg, a->g, s->d_gbias, pl.L, pl.G, c.gin_channels);
+        h->launches++;
+    }
+    if (cudaStreamSynchronize(st) != cudaSuccess || cudaGetLastError() != cudaSuccess)
+        return bail(fail(WN_ERR_CUDA, "stream set-up failed"));
+    *stream = s;
+    return WN_OK;
+}
+
+int32_t wn_stream_generate(void* stream, const wn_generate_args* chunk, const wn_stream_chunk* where) {
+    WnStream* s = (WnStream*)stream;
+    if (!s || !chunk) return fail(WN_ERR_INVALID, "null argument");
+    WnHandle* h = s->h;
+    if (s->final) return fail(WN_ERR_STATE, "the stream was finalised: no chunk may follow its final one");
+    if (h->weight_gen != s->weight_gen)
+        return fail(WN_ERR_STATE, "the handle's weights changed since the stream was opened (wn_load_weights)");
+    if (chunk->B != s->B) return fail(WN_ERR_INVALID, "chunk B differs from the B the stream was opened with");
+    if (chunk->g || chunk->initial || chunk->initial_rows || chunk->initial_dense)
+        return fail(WN_ERR_INVALID, "g and the initial input belong to wn_stream_open, not to a chunk");
+    if (chunk->T_test != 0 || chunk->test_scalar || chunk->test_index || chunk->test_dense)
+        return fail(WN_ERR_INVALID, "teacher forcing is not supported in a stream");
+    if (chunk->T >= 1 && s->t + chunk->T > (1LL << 32))
+        return fail(WN_ERR_INVALID, "absolute step beyond 2^32 (the Philox step counter is 32-bit)");
+    wn_generate_args a = *chunk;
+    a.initial = s->open.initial;
+    a.initial_index = s->open.initial_index;
+    a.initial_rows = s->open.initial_rows;
+    a.initial_dense = s->open.initial_dense;
+    a.flags = s->open.flags;
+    a.noise_kind = s->open.noise_kind;
+    a.seed = s->open.seed;
+    a.philox_row0 = s->open.philox_row0;
+    int32_t rc = validate_args(h, &a, true);
+    if (rc) return rc;
+    DeviceGuard guard(h->cfg.device);
+    cudaStream_t st = (cudaStream_t)a.stream;
+    if (a.c_frames) {
+        if (!where) return fail(WN_ERR_INVALID, "c_frames in a stream needs its wn_stream_chunk (frame offset, frames so far)");
+        if (where->frame_offset < 0 || a.n_frames < 1 || where->frame_offset + a.n_frames > where->frames_total)
+            return fail(WN_ERR_INVALID, "the frame window lies outside the frames received so far");
+        long long f_lo, f_hi, n_ready;
+        rc = ups_cone(h->ups, h->ups_total, h->ups_ks, where->frames_total, where->final != 0, 0, 0, &f_lo, &f_hi,
+                      &n_ready);
+        if (rc) return rc;
+        if (s->t + a.T > n_ready)
+            return fail(WN_ERR_INVALID, "samples [" + std::to_string(s->t) + "," + std::to_string(s->t + a.T) +
+                                            ") are not known yet from " + std::to_string(where->frames_total) +
+                                            " frames (" + std::to_string(n_ready) + " are)");
+        rc = ups_cone(h->ups, h->ups_total, h->ups_ks, where->frames_total, where->final != 0, s->t, s->t + a.T, &f_lo,
+                      &f_hi, &n_ready);
+        if (rc) return rc;
+        if (f_lo < where->frame_offset || f_hi > where->frame_offset + a.n_frames)
+            return fail(WN_ERR_INVALID, "the frame window [" + std::to_string(where->frame_offset) + "," +
+                                            std::to_string(where->frame_offset + a.n_frames) + ") does not cover frames [" +
+                                            std::to_string(f_lo) + "," + std::to_string(f_hi) + ") the chunk needs");
+        const int lost = h->ups_ks > 0 ? h->ups_ks - 1 : 0;
+        const int n0 = where->final ? (int)(where->frames_total - lost) : WNAUX_UNBOUNDED;
+        rc = run_upsampler(h, a.c_frames, a.B, a.n_frames, a.T, st, (int)where->frame_offset, n0, (int)s->t);
+        if (rc) return rc;
+        a.c = h->d_cup;
+        a.c_frames = nullptr;
+    }
+    StreamCtx sc;
+    sc.state = s->d_state;
+    sc.state_load = s->t > 0 ? 1 : 0;
+    sc.t_base = (unsigned)s->t;
+    sc.gbias = s->d_gbias;
+    rc = launch_chunk(h, &a, 0, a.B, st, &sc);
+    if (rc) return rc;
+    s->t += a.T;
+    if (where && where->final) s->final = true;
+    h->last_stream = st;
+    h->pending = true;
+    return WN_OK;
+}
+
+int64_t wn_stream_position(void* stream) {
+    WnStream* s = (WnStream*)stream;
+    return s ? (int64_t)s->t : (int64_t)fail(WN_ERR_INVALID, "null stream");
+}
+
+int32_t wn_stream_close(void* stream) {
+    WnStream* s = (WnStream*)stream;
+    if (!s) return WN_OK;
+    DeviceGuard guard(s->h->cfg.device);
+    cudaDeviceSynchronize();           // a chunk in flight still reads and writes the state
+    cudaFree(s->d_state);
+    cudaFree(s->d_gbias);
+    cudaFree(s->d_init);
+    delete s;
     return WN_OK;
 }
 

@@ -87,7 +87,19 @@ struct WnPtrs {
     int warp_reverse;          // 1: logical warp = 9 - physical warp (the issue arbiter favours high warp ids)
     int gate_cycles;           // the critical group does not poll an exchange earlier than this after its own publish
     int fast_gate;             // 1: approximate exponentials / division in the gate of the lean stage path
+    // ---- streaming (wn_stream_generate): a launch continues an utterance at absolute step t_base
+    unsigned t_base;           // absolute step of local step 0 (Philox counters, ring positions); 0 for a whole utterance
+    float* state;              // NULL, or [P][ring floats] rings then the feedback [BT] s_in, [BT] s_idx, [BT][O] s_dense
+    int state_load;            // 1: rings and step-0 feedback come from `state`; 0: zero rings, feedback from initial*
 };
+
+// floats of the stream state that follow the rings: the feedback of the next step
+__host__ __device__ inline long long wn_state_feedback_floats(const WnPlan& pl) {
+    return 2LL * pl.BT + (pl.input_kind != 0 ? (long long)pl.BT * pl.O : 0);
+}
+__host__ __device__ inline long long wn_state_ring_floats(const WnPlan& pl) {
+    return (long long)pl.ring_pos_total * pl.RA4 * pl.BT;       // per block
+}
 
 #define WN_FLAG_SOFTMAX_ 1u
 #define WN_FLAG_QUANTIZE_ 2u
@@ -345,8 +357,11 @@ __device__ __noinline__ bool wn_wait_count_slow(volatile int* cnt, int need, uns
 
 // LEAN: the lean stage path (crit_loop / def_loop) INSTEAD of the generic one -- a separate, smaller kernel: compiled
 // into the same kernel the two paths cost each other registers and instruction-cache footprint, which slows the
-// generic path with the lean code merely present
-template <int BT, int ER, int EG, bool LEAN = false>
+// generic path with the lean code merely present.
+// STREAM: the kernel of wn_stream_generate (absolute steps, history and feedback in a state buffer).  A separate
+// instantiation too: any code after the step loops changes the register allocation of the loops (the config-2 kernel
+// then spills in its hot loop and loses 9 % on an H100 SXM at 400 W), so the whole-utterance kernels compile as before.
+template <int BT, int ER, int EG, bool LEAN = false, bool STREAM = false>
 struct Engine {
     static_assert(!LEAN || (BT == 1 && ER % 2 == 0 && EG % 2 == 0), "lean path: one utterance, paired elements");
     static constexpr int NV = 4 * BT;
@@ -753,6 +768,7 @@ struct Engine {
         const uint32_t ub = (uint32_t)(pp.b0 + b);
         const bool replay = pp.noise_kind == 0;
         const uint2 key = make_uint2((uint32_t)pp.seed, (uint32_t)(pp.seed >> 32));
+        const uint32_t tc = (STREAM ? pp.t_base : 0u) + (uint32_t)t;   // Philox counts absolute steps; replay is per launch
         if (b >= pp.B) {   // padding row of the batch tile: harmless constants
             for (int i = lane; i < O + 2; i += 32) nz[i] = 0.5f;
             return;
@@ -762,7 +778,7 @@ struct Engine {
                 float e;
                 if (replay) e = pp.e ? __ldg(pp.e + ((size_t)t * B + b) * O + i) : 1.0f;
                 else {
-                    const uint4 r = philox4(make_uint4((uint32_t)t, ub, (uint32_t)i, 2u), key);
+                    const uint4 r = philox4(make_uint4(tc, ub, (uint32_t)i, 2u), key);
                     e = -logf(u01(r.x));
                 }
                 nz[i] = e;
@@ -774,7 +790,7 @@ struct Engine {
             for (int i = lane; i < K; i += 32) {
                 float u;
                 if (replay) u = __ldg(pp.u1 + ((size_t)t * B + b) * K + i);
-                else u = u01(philox4(make_uint4((uint32_t)t, ub, (uint32_t)i, 0u), key).x);
+                else u = u01(philox4(make_uint4(tc, ub, (uint32_t)i, 0u), key).x);
                 nz[i] = u;
             }
         }
@@ -782,11 +798,11 @@ struct Engine {
             float v;
             if (pl.head_kind == 0) {
                 if (replay) v = __ldg(pp.u2 + (size_t)t * B + b);
-                else v = u01(philox4(make_uint4((uint32_t)t, ub, 0u, 1u), key).x);
+                else v = u01(philox4(make_uint4(tc, ub, 0u, 1u), key).x);
             } else {
                 if (replay) v = __ldg(pp.z + (size_t)t * B + b);
                 else {
-                    const uint4 r = philox4(make_uint4((uint32_t)t, ub, 0u, 1u), key);
+                    const uint4 r = philox4(make_uint4(tc, ub, 0u, 1u), key);
                     v = sqrtf(-2.f * logf(u01(r.x))) * cospif(2.f * u01(r.y));   // Box-Muller
                 }
             }
@@ -1696,13 +1712,43 @@ struct Engine {
 };
 
 // ------------------------------------------------------------------------------------------
+// Stream epilogue (compute threads only).  Both loops end every step on a group barrier after the deferred group's
+// ring writes and the sampler's feedback, so the rings and the feedback of step T are final here.  Nothing else
+// carries over a step: skipacc restarts at layer 0, stash / partials / pre-sums are per stage.
+// ------------------------------------------------------------------------------------------
+template <int BT>
+__device__ __noinline__ void wn_store_state(const WnPlan& pl, const WnPtrs& pp, unsigned char* sm) {
+    const int warp = pp.warp_reverse ? (WN_NTHREADS / 32 - 1) - (int)(threadIdx.x >> 5) : (int)(threadIdx.x >> 5);
+    const int tid = warp * 32 + (int)(threadIdx.x & 31), p = blockIdx.x;
+    if (tid >= WN_NT) return;
+    const long long ring_n = wn_state_ring_floats(pl);
+    if (pl.ring_in_smem) {
+        const volatile float* ring = reinterpret_cast<const volatile float*>(sm + pl.sm_ring);
+        float* dst = pp.state + (size_t)p * ring_n;
+        for (long long i = tid; i < ring_n; i += WN_NT) dst[i] = ring[i];
+    }
+    if (p == 0) {
+        const float* s_in = reinterpret_cast<const float*>(sm + pl.sm_in);      // layout of Engine's s_in / s_idx / s_dense
+        const int* s_idx = reinterpret_cast<const int*>(s_in + BT);
+        const float* s_dense = reinterpret_cast<const float*>(s_idx + BT);
+        float* fb = pp.state + (size_t)pl.P * ring_n;
+        for (int b = tid; b < BT; b += WN_NT) {
+            fb[b] = s_in[b];
+            fb[BT + b] = __int_as_float(s_idx[b]);
+        }
+        if (pl.input_kind != 0)
+            for (int i = tid; i < BT * pl.O; i += WN_NT) fb[2 * BT + i] = s_dense[i];
+    }
+}
+
+// ------------------------------------------------------------------------------------------
 // kernel entry
 // ------------------------------------------------------------------------------------------
-template <int BT, int ER, int EG, bool LEAN = false>
+template <int BT, int ER, int EG, bool LEAN = false, bool STREAM = false>
 __global__ void __launch_bounds__(WN_NTHREADS, 1)
 wn_persistent_kernel(const __grid_constant__ WnPlan pl, const __grid_constant__ WnPtrs pp) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
-    Engine<BT, ER, EG, LEAN> eng(pl, pp, smem_raw);
+    Engine<BT, ER, EG, LEAN, STREAM> eng(pl, pp, smem_raw);
     const int tid = eng.tid, p = blockIdx.x;      // logical thread index (see Engine)
     const int nslots = pl.nres + pl.nring;
     if (tid == 0) {
@@ -1717,16 +1763,18 @@ wn_persistent_kernel(const __grid_constant__ WnPlan pl, const __grid_constant__ 
         *eng.s_ddone_cnt = 0;
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    // zero the history (== the reference's zero-initialised queue, conv.py:35-36) and scratch
+    // zero the history (== the reference's zero-initialised queue, conv.py:35-36) and scratch; a continued stream
+    // loads the history its previous launch stored instead (rings in global memory ARE the state buffer: nothing to do)
+    const long long ring_n = wn_state_ring_floats(pl);
     if (pl.ring_in_smem) {
-        const size_t n = (size_t)pl.ring_pos_total * pl.RA4 * BT;
-        for (size_t i = tid; i < n; i += WN_NTHREADS) eng.ring[i] = 0.f;
+        const float* src = (STREAM && pp.state_load) ? pp.state + (size_t)p * ring_n : nullptr;
+        for (long long i = tid; i < ring_n; i += WN_NTHREADS) eng.ring[i] = src ? src[i] : 0.f;
     }
     for (int i = tid; i < pl.NSm * BT + 4; i += WN_NTHREADS) eng.skipacc[i] = 0.f;
     for (int i = tid; i < pl.L * (pl.kw - 1); i += WN_NTHREADS) {
         eng.ringtab[i * 3] = pp.ringtab[i * 2];           // offset of the ring (in positions)
         eng.ringtab[i * 3 + 1] = pp.ringtab[i * 2 + 1];   // delay D
-        eng.ringtab[i * 3 + 2] = 0;                       // t mod D
+        eng.ringtab[i * 3 + 2] = STREAM ? (int)(pp.t_base % (unsigned)pp.ringtab[i * 2 + 1]) : 0;   // (absolute t) mod D
     }
     for (int k = tid; k < pl.R; k += WN_NTHREADS) {
         eng.first[k] = (pl.input_kind == 0) ? pp.first_w[k] : 0.f;
@@ -1768,17 +1816,19 @@ wn_persistent_kernel(const __grid_constant__ WnPlan pl, const __grid_constant__ 
                 else idx = pp.initial_index;
             }
         } else if (pl.input_kind != 0) idx = 0;
-        eng.s_in[b] = v;
-        eng.s_idx[b] = idx;
+        const float* fb = (STREAM && pp.state_load) ? pp.state + (size_t)pl.P * ring_n : nullptr;   // the last launch's
+        eng.s_in[b] = fb ? fb[b] : v;
+        eng.s_idx[b] = fb ? __float_as_int(fb[BT + b]) : idx;
     }
     if (pl.input_kind != 0) {
         const float* dsrc = nullptr;
         size_t stride = 0;
         if (pp.T_test > 0 && pp.test_dense != nullptr) { dsrc = pp.test_dense; stride = (size_t)pp.T_test * pl.O; }
         else if (pp.T_test == 0 && pp.initial_dense != nullptr) { dsrc = pp.initial_dense; stride = (size_t)pl.O; }
+        const float* fb = (STREAM && pp.state_load) ? pp.state + (size_t)pl.P * ring_n + 2 * BT : nullptr;
         for (int i = tid; i < BT * pl.O; i += WN_NTHREADS) {
             const int b = i / pl.O, o = i % pl.O;
-            eng.s_dense[i] = (dsrc && b < pp.B) ? dsrc[(size_t)b * stride + o] : 0.f;
+            eng.s_dense[i] = fb ? fb[i] : ((dsrc && b < pp.B) ? dsrc[(size_t)b * stride + o] : 0.f);
         }
     }
     const int warp = tid >> 5;
@@ -1794,6 +1844,7 @@ wn_persistent_kernel(const __grid_constant__ WnPlan pl, const __grid_constant__ 
     }
     if (warp < WN_GW) eng.crit_loop();
     else eng.def_loop();
+    if constexpr (STREAM) wn_store_state<BT>(pl, pp, smem_raw);
 }
 
 // gbias[b][l][row] = Wg_l[row,:] . g_b   (modules.py:148-152), once per call

@@ -67,6 +67,62 @@ def decode_device(y_hat: torch.Tensor, lengths: Optional[Sequence[int]] = None, 
     return (pcm, flt) if want_float else pcm
 
 
+class StreamDecoder:
+    """``decode_device`` chunk by chunk: feed consecutive chunks (B,C,T_i) of the model output and get each chunk's
+    int16 (and, with ``want_float``, float) waveform; the concatenation equals one ``decode_device`` call over the
+    whole output bit for bit.  The inv_preemphasis recursion carries over chunk boundaries on the device
+    (wn_decode_stream); ``lengths`` are the utterances' lengths in the whole output."""
+
+    def __init__(self, B: int, device, input_type: str = "raw", quantize_channels: int = 65536,
+                 postprocess: Optional[str] = None, global_gain_scale: float = 0.0, preemphasis_coef: float = 0.85,
+                 lengths: Optional[Sequence[int]] = None, want_float: bool = False):
+        device = torch.device(device)
+        if device.type != "cuda":
+            raise RuntimeError("StreamDecoder runs on a CUDA device only (no CPU fallback)")
+        if device.index is None:
+            device = torch.device("cuda", torch.cuda.current_device())
+        if postprocess not in (None, "", "none", "inv_preemphasis"):
+            raise ValueError("unsupported postprocess %r" % (postprocess,))
+        self.B, self.device = int(B), device
+        self.kind = INPUT_TYPES[input_type]
+        self.quantize_channels = int(quantize_channels)
+        self.coef = float(preemphasis_coef) if postprocess == "inv_preemphasis" else 0.0
+        self.gain = float(global_gain_scale)
+        self.lengths = None if lengths is None else [int(v) for v in lengths]
+        self.want_float = bool(want_float)
+        self.carry = torch.zeros(self.B, dtype=torch.float32, device=device)   # coef * last sample of the previous chunk
+        self.t = 0
+
+    def __call__(self, y_hat: torch.Tensor):
+        import ctypes as C
+        from . import _native as N
+        B = self.B
+        if y_hat.device != self.device or y_hat.size(0) != B:
+            raise ValueError("expected a (%d,C,T) chunk on %s" % (B, self.device))
+        y_s = y_i = None
+        if self.kind == 2:
+            y_i = y_hat.max(1)[1].view(B, -1).to(torch.int32).contiguous()      # synthesis.py:68
+            T = y_i.size(1)
+        else:
+            y_s = y_hat.reshape(B, -1).float().contiguous()
+            T = y_s.size(1)
+        pcm = torch.empty(B, T, dtype=torch.int16, device=self.device)
+        flt = torch.empty(B, T, dtype=torch.float32, device=self.device) if self.want_float else None
+        if T == 0:
+            return (pcm, flt) if self.want_float else pcm
+        len_t = None
+        if self.lengths is not None:
+            len_t = torch.tensor([max(0, v - self.t) for v in self.lengths], dtype=torch.int32, device=self.device)
+        with torch.cuda.device(self.device):
+            N.check(N.lib().wn_decode_stream(None if y_s is None else y_s.data_ptr(), None if y_i is None else y_i.data_ptr(),
+                                             B, T, None if len_t is None else len_t.data_ptr(), self.kind,
+                                             self.quantize_channels, C.c_float(self.coef), C.c_float(self.gain),
+                                             None if flt is None else flt.data_ptr(), pcm.data_ptr(), self.carry.data_ptr(),
+                                             torch.cuda.current_stream(self.device).cuda_stream))
+        self.t += T
+        return (pcm, flt) if self.want_float else pcm
+
+
 def list_feature_files(data_dir: str) -> List[str]:
     files = sorted(glob(os.path.join(data_dir, "*-feats.npy")))
     if not files:

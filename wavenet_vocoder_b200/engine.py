@@ -9,6 +9,7 @@ optional teacher-forcing inputs, and returns the generated samples.
 from __future__ import annotations
 
 import ctypes as C
+import weakref
 from typing import Dict, Optional
 
 import torch
@@ -98,6 +99,182 @@ def make_config(*, layers, stacks, residual_channels, gate_channels, skip_out_ch
     return cfg
 
 
+def upsampler_struct(net, cin):
+    """The wn_upsampler of a PyTorch upsample network (upsample.py), or None for a variant the native path does not
+    cover.  Returns {"u": wn_upsampler, "total", "frames_lost", "indent"}; the struct's arrays are kept in the dict."""
+    from . import upsample as U
+    if net is None or cin <= 0:
+        return None
+    conv_in = None
+    up = net
+    if isinstance(net, U.ConvInUpsampleNetwork):
+        conv_in, up = net.conv_in, net.upsample
+    if not isinstance(up, U.UpsampleNetwork):
+        return None
+    scales, filters = [], []
+    layers = list(up.up_layers)
+    if len(layers) % 2 != 0:
+        return None                                    # an activation follows every conv
+    for st, conv in zip(layers[0::2], layers[1::2]):
+        if not isinstance(st, U.Stretch2d) or st.mode != "nearest" or st.y_scale != 1:
+            return None
+        sd = {k: v for k, v in conv.state_dict().items()}
+        if "weight" in sd:
+            w = sd["weight"].detach().float().cpu()
+        else:
+            w = torch._weight_norm(sd["weight_v"].detach().float().cpu(), sd["weight_g"].detach().float().cpu(), 0)
+        s = int(st.x_scale)
+        if w.shape != (1, 1, 1, 2 * s + 1) or s < 2:
+            return None
+        scales.append(s)
+        filters.append(w.reshape(-1))
+    if not scales or len(scales) > 8:
+        return None
+    u = N.wn_upsampler()
+    u.channels = cin
+    u.n_scales = len(scales)
+    sc = (C.c_int32 * len(scales))(*scales)
+    fl = torch.cat(filters).contiguous()
+    u.scales = sc
+    u.filters = C.cast(fl.data_ptr(), C.POINTER(C.c_float))
+    cw = None
+    if conv_in is not None:
+        cw = conv_in.weight.detach().float().cpu().contiguous()
+        if cw.shape[0] != cin or cw.shape[1] != cin or conv_in.bias is not None:
+            return None
+        u.conv_in_w = C.cast(cw.data_ptr(), C.POINTER(C.c_float))
+        u.conv_in_ks = int(cw.shape[2])
+    u.indent = int(up.indent)
+    total = 1
+    for s in scales:
+        total *= s
+    return dict(u=u, keep=(sc, fl, cw), total=total, frames_lost=int(cw.shape[2]) - 1 if cw is not None else 0,
+                indent=int(up.indent))
+
+
+def upsample_cone(u, n_frames, final, t_lo=0, t_hi=0):
+    """wn_upsample_cone (no device needed): (f_lo, f_hi, n_ready)."""
+    f_lo, f_hi, n_ready = C.c_int64(), C.c_int64(), C.c_int64()
+    N.check(N.lib().wn_upsample_cone(C.byref(u), int(n_frames), int(bool(final)), int(t_lo), int(t_hi), C.byref(f_lo),
+                                     C.byref(f_hi), C.byref(n_ready)))
+    return f_lo.value, f_hi.value, n_ready.value
+
+
+class SynthesisStream:
+    """One utterance (or one batch tile of them) made chunk by chunk; the state between chunks stays on the device
+    (wn_stream_* of include/wn.h).  Chunks are bit-identical to the same samples of one ``generate`` call."""
+
+    def __init__(self, eng, *, B, g=None, initial=None, initial_index=-1, initial_rows=None, initial_dense=None,
+                 softmax=True, quantize=True, replay=False, seed=None, philox_row0=0):
+        self.eng, self.B, self.quantize = eng, int(B), bool(quantize)
+        dev = eng.device
+        a = N.wn_stream_open_args()
+        a.B = self.B
+        hold = []
+
+        def dptr(t, dtype=torch.float32, shape=None):
+            if t is None:
+                return None
+            t = t.to(device=dev, dtype=dtype).contiguous()
+            if shape is not None and tuple(t.shape) != tuple(shape):
+                raise ValueError("expected shape %s, got %s" % (tuple(shape), tuple(t.shape)))
+            hold.append(t)
+            return t.data_ptr()
+
+        a.g = dptr(g, shape=(B, eng.gin) if g is not None else None)
+        a.initial = dptr(initial, shape=(B,) if initial is not None else None)
+        a.initial_index = int(initial_index)
+        a.initial_rows = dptr(initial_rows, torch.int32, shape=(B,) if initial_rows is not None else None)
+        a.initial_dense = dptr(initial_dense, shape=(B, eng.out_channels) if initial_dense is not None else None)
+        a.flags = (N.WN_FLAG_SOFTMAX if softmax else 0) | (N.WN_FLAG_QUANTIZE if quantize else 0)
+        if replay:
+            a.noise_kind = N.WN_NOISE_REPLAY
+        else:
+            a.noise_kind = N.WN_NOISE_PHILOX
+            if seed is None:
+                seed = int(torch.randint(0, 2 ** 62, (1,), dtype=torch.int64).item())
+            a.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
+        a.philox_row0 = int(philox_row0)
+        a.stream = torch.cuda.current_stream(dev).cuda_stream
+        self._s = C.c_void_p()
+        N.check(N.lib().wn_stream_open(eng._h, C.byref(a), C.byref(self._s)))   # returns after the set-up ran
+        eng._streams.add(self)
+
+    @property
+    def t(self) -> int:
+        """Samples generated so far (the absolute step of the next one)."""
+        self._check_open()
+        return int(N.lib().wn_stream_position(self._s))
+
+    def _check_open(self):
+        if not self._s.value:
+            raise RuntimeError("the stream is closed")
+
+    def generate(self, T, *, c=None, c_frames=None, frame_offset=0, frames_total=0, final=False, noise=None,
+                 want_params=False, sync=True):
+        """The next T samples.  c: (B,T,C) sample-rate conditioning of these samples; or c_frames (B,C,n), utterance
+        frames [frame_offset, frame_offset+n) of the frames_total received so far (``final``: all of them).
+        noise: these T steps' replayed draws, (T,B,.).  Returns (out, params) as SynthesisEngine.generate."""
+        self._check_open()
+        eng, B, dev, O = self.eng, self.B, self.eng.device, self.eng.out_channels
+        a = N.wn_generate_args()
+        a.B, a.T = B, int(T)
+        hold = []
+
+        def dptr(t, shape=None):
+            if t is None:
+                return None
+            t = t.to(device=dev, dtype=torch.float32).contiguous()
+            if shape is not None and tuple(t.shape) != tuple(shape):
+                raise ValueError("expected shape %s, got %s" % (tuple(shape), tuple(t.shape)))
+            hold.append(t)
+            return t.data_ptr()
+
+        a.c = dptr(c, shape=(B, T, eng.cin) if c is not None else None)
+        where = None
+        if c_frames is not None:
+            a.c_frames = dptr(c_frames, shape=(B, eng.cin, c_frames.size(-1)))
+            a.n_frames = int(c_frames.size(-1))
+        if c_frames is not None or final:
+            where = N.wn_stream_chunk()
+            where.frame_offset, where.frames_total, where.final = int(frame_offset), int(frames_total), int(bool(final))
+        if noise is not None:
+            a.noise_u1 = dptr(noise.get("u1"), shape=(T, B, eng.K) if "u1" in noise else None)
+            a.noise_u2 = dptr(noise.get("u2"), shape=(T, B) if "u2" in noise else None)
+            a.noise_z = dptr(noise.get("z"), shape=(T, B) if "z" in noise else None)
+            a.noise_e = dptr(noise.get("e"), shape=(T, B, O) if "e" in noise else None)
+        if eng.scalar_input:
+            out = torch.empty(B, T, device=dev, dtype=torch.float32)
+            a.out_scalar = out.data_ptr()
+        elif self.quantize:
+            out = torch.empty(B, T, device=dev, dtype=torch.int32)
+            a.out_index = out.data_ptr()
+        else:
+            out = torch.empty(B, O, T, device=dev, dtype=torch.float32)
+            a.out_dense = out.data_ptr()
+        params = None
+        if want_params:
+            params = torch.empty(B, O, T, device=dev, dtype=torch.float32)
+            a.params_out = params.data_ptr()
+        a.stream = torch.cuda.current_stream(dev).cuda_stream
+        N.check(N.lib().wn_stream_generate(self._s, C.byref(a), None if where is None else C.byref(where)))
+        eng._keep = hold
+        if sync:
+            eng.sync()
+        return out, params
+
+    def close(self):
+        if getattr(self, "_s", None) is not None and self._s.value:
+            N.lib().wn_stream_close(self._s)
+            self._s = C.c_void_p()
+            self.eng._streams.discard(self)
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
 
 class SynthesisEngine:
     """One model shape on one GPU."""
@@ -133,8 +310,12 @@ class SynthesisEngine:
         self._sd = None
         self._halves = None           # two half-grid engines for concurrent batch tiles (see generate_concurrent)
         self._is_child = num_ctas > 0
+        self._ups = None
+        self._streams = weakref.WeakSet()   # open SynthesisStreams: closed before the handle they run on
 
     def close(self):
+        for s in list(getattr(self, "_streams", None) or []):
+            s.close()
         for ch in (getattr(self, "_halves", None) or []):
             ch["eng"].close()
         self._halves = None
@@ -165,62 +346,29 @@ class SynthesisEngine:
         raw conditioning frames.  Returns False (and unloads) for variants the native path does not cover
         (freq_axis_kernel_size != 1, an activation, a non-nearest mode, a scale < 2): the caller then keeps
         them on the PyTorch side and passes sample-rate ``c``."""
-        from . import upsample as U
         self._ups_net = net
         for ch in (getattr(self, "_halves", None) or []):
             ch["eng"].load_upsampler(net)
         self.ups_frames_lost = 0
         self.ups_total = 1
+        self._ups = None
         N.check(N.lib().wn_load_upsampler(self._h, None))
-        if net is None or self.cin <= 0:
+        d = upsampler_struct(net, self.cin)
+        if d is None:
             return False
-        conv_in = None
-        up = net
-        if isinstance(net, U.ConvInUpsampleNetwork):
-            conv_in, up = net.conv_in, net.upsample
-        if not isinstance(up, U.UpsampleNetwork):
-            return False
-        scales, filters = [], []
-        layers = list(up.up_layers)
-        if len(layers) % 2 != 0:
-            return False                                   # an activation follows every conv
-        for st, conv in zip(layers[0::2], layers[1::2]):
-            if not isinstance(st, U.Stretch2d) or st.mode != "nearest" or st.y_scale != 1:
-                return False
-            sd = {k: v for k, v in conv.state_dict().items()}
-            if "weight" in sd:
-                w = sd["weight"].detach().float().cpu()
-            else:
-                w = torch._weight_norm(sd["weight_v"].detach().float().cpu(), sd["weight_g"].detach().float().cpu(), 0)
-            s = int(st.x_scale)
-            if w.shape != (1, 1, 1, 2 * s + 1) or s < 2:
-                return False
-            scales.append(s)
-            filters.append(w.reshape(-1))
-        if not scales or len(scales) > 8:
-            return False
-        u = N.wn_upsampler()
-        u.channels = self.cin
-        u.n_scales = len(scales)
-        sc = (C.c_int32 * len(scales))(*scales)
-        fl = torch.cat(filters).contiguous()
-        u.scales = sc
-        u.filters = C.cast(fl.data_ptr(), C.POINTER(C.c_float))
-        cw = None
-        if conv_in is not None:
-            cw = conv_in.weight.detach().float().cpu().contiguous()
-            if cw.shape[0] != self.cin or cw.shape[1] != self.cin or conv_in.bias is not None:
-                return False
-            u.conv_in_w = C.cast(cw.data_ptr(), C.POINTER(C.c_float))
-            u.conv_in_ks = int(cw.shape[2])
-        u.indent = int(up.indent)
-        N.check(N.lib().wn_load_upsampler(self._h, C.byref(u)))
-        self.ups_total = 1
-        for s in scales:
-            self.ups_total *= s
-        self.ups_frames_lost = (int(cw.shape[2]) - 1 if cw is not None else 0)
-        self.ups_indent = int(up.indent)
+        N.check(N.lib().wn_load_upsampler(self._h, C.byref(d["u"])))
+        self._ups = d
+        self.ups_total = d["total"]
+        self.ups_frames_lost = d["frames_lost"]
+        self.ups_indent = d["indent"]
         return True
+
+    def upsample_cone(self, n_frames: int, final: bool, t_lo: int = 0, t_hi: int = 0):
+        """(f_lo, f_hi, n_ready): the frames [f_lo, f_hi) samples [t_lo, t_hi) need, and how many samples from the
+        start are known from ``n_frames`` frames (``final``: all of them); libwn's wn_upsample_cone."""
+        if self._ups is None:
+            raise RuntimeError("no native upsampler is loaded")
+        return upsample_cone(self._ups["u"], n_frames, final, t_lo, t_hi)
 
     def upsample(self, c_frames: torch.Tensor, T: int) -> torch.Tensor:
         """(B,C,frames) -> (B,T,C): only the upsampler of libwn (tests / tools)."""
@@ -320,6 +468,11 @@ class SynthesisEngine:
         if sync:
             self.sync()
         return out, params
+
+    # ------------------------------------------------------------------ streaming
+    def open_stream(self, **kw) -> SynthesisStream:
+        """A stream of chunks on this handle (keywords of SynthesisStream); one batch tile, engine 5."""
+        return SynthesisStream(self, **kw)
 
     # ------------------------------------------------------------------ two batch tiles at a time
     def generate_concurrent(self, *, B: int, T: int, c: Optional[torch.Tensor] = None,

@@ -336,3 +336,135 @@ class WaveNet(nn.Module):
         else:
             y = out
         return (y, params) if return_params else y
+
+    # ------------------------------------------------------------------ streaming
+    @torch.no_grad()
+    def open_stream(self, B=1, g=None, initial_input=None, seed=None, noise=None, softmax=True, quantize=True,
+                    return_params=False):
+        """Synthesis in chunks: a ``WaveNetStream`` whose chunks concatenate to exactly what ``incremental_forward``
+        returns for the whole utterance with the same ``g``, ``initial_input``, ``seed`` or ``noise`` (the whole
+        utterance's replayed draws, sliced per chunk) and conditioning.  The state between chunks (history queues,
+        fed-back sample, noise position) stays on the device.  At most one batch tile (4 utterances); no teacher
+        forcing; engine 5."""
+        if self.training:
+            raise RuntimeError("open_stream only supports eval mode")
+        return WaveNetStream(self, B=int(B), g=g, initial_input=initial_input, seed=seed, noise=noise,
+                             softmax=softmax, quantize=quantize, return_params=return_params)
+
+
+class WaveNetStream:
+    """Chunks of one utterance (or a batch tile of them) from ``WaveNet.open_stream``.
+
+    ``generate(T, c=)`` takes sample-rate conditioning; ``push_frames(frames)`` takes conditioning frames as they
+    arrive and returns the samples whose frames are all known (possibly none); ``finish()`` returns the rest, up to
+    the upsampled length of all frames pushed.  Outputs are laid out as ``incremental_forward``'s."""
+
+    def __init__(self, model, *, B, g, initial_input, seed, noise, softmax, quantize, return_params):
+        self._m = model
+        self._eng = eng = model._get_engine()
+        dev = eng.device
+        O = model.out_channels
+        g_vec = None
+        if g is not None:
+            g = g.to(dev)
+            if model.embed_speakers is not None:
+                g_vec = model.embed_speakers(g.view(g.size(0), -1).long())[:, 0, :]   # wavenet.py:263-266
+            else:
+                g_vec = g.reshape(g.size(0), -1).float()
+            if g_vec.size(0) == 1 and B > 1:
+                g_vec = g_vec.expand(B, -1)
+        initial = initial_rows = initial_dense = None
+        if initial_input is not None:
+            ii = initial_input.to(dev).float()
+            if model.scalar_input:
+                initial = ii.reshape(ii.size(0), -1)[:, 0]
+                initial = initial.expand(B) if initial.size(0) == 1 else initial
+            else:
+                if ii.size(1) == O and ii.size(-1) != O:
+                    ii = ii.transpose(1, 2)
+                first = ii.reshape(ii.size(0), -1, O)[:, 0]
+                first = first.expand(B, -1) if first.size(0) == 1 else first
+                idx = first.argmax(-1)
+                if torch.equal(torch.zeros_like(first).scatter_(-1, idx.unsqueeze(-1), 1.0), first):
+                    initial_rows = idx.to(torch.int32)
+                else:
+                    initial_dense = first
+        self._noise = None if noise is None else {k: v.to(dev) for k, v in noise.items()}
+        self._s = eng.open_stream(B=B, g=g_vec, initial=initial, initial_rows=initial_rows, initial_dense=initial_dense,
+                                  softmax=bool(softmax), quantize=bool(quantize), replay=noise is not None, seed=seed)
+        self.B, self._quantize, self._return_params = B, bool(quantize), bool(return_params)
+        self._frames = None          # every frame pushed so far, (B,C,n) on the device
+        self._finished = False
+
+    @property
+    def t(self) -> int:
+        """Samples generated so far."""
+        return self._s.t
+
+    def close(self):
+        self._s.close()
+
+    def _chunk(self, T, **kw):
+        if self._finished:
+            raise RuntimeError("the stream was finished")
+        if self._m._get_engine() is not self._eng:      # reloads changed weights: the library then refuses the chunk
+            raise RuntimeError("the model moved to another device since the stream was opened")
+        t = self.t
+        noise = None if self._noise is None else {k: v[t:t + T] for k, v in self._noise.items()}
+        out, params = self._s.generate(T, noise=noise, want_params=self._return_params, **kw)
+        B, O = self.B, self._m.out_channels
+        if self._m.scalar_input:
+            y = out.view(B, 1, T)
+        elif self._quantize:
+            y = torch.zeros(B, O, T, device=out.device).scatter_(1, out.long().unsqueeze(1), 1.0)
+        else:
+            y = out
+        return (y, params) if self._return_params else y
+
+    def _empty(self):
+        dev = self._eng.device
+        C = 1 if self._m.scalar_input else self._m.out_channels
+        y = torch.zeros(self.B, C, 0, device=dev)
+        return (y, torch.zeros(self.B, self._m.out_channels, 0, device=dev)) if self._return_params else y
+
+    @torch.no_grad()
+    def generate(self, T, c=None):
+        """The next T samples; ``c``: their sample-rate conditioning, (B,C,T) or (B,T,C)."""
+        T = int(T)
+        if c is not None:
+            c = c.to(self._eng.device).float()
+            if c.size(-1) == T and c.size(1) == self._m.cin_channels:
+                c = c.transpose(1, 2)
+            c = c.contiguous()
+        return self._chunk(T, c=c)
+
+    @torch.no_grad()
+    def push_frames(self, frames):
+        """Append conditioning frames (B,C,n) and return the samples they complete (possibly none)."""
+        frames = frames.to(self._eng.device).float()
+        if self._m.upsample_net is None:
+            return self.generate(frames.size(-1), c=frames)       # frames are at the sample rate already
+        if not self._m._native_upsample:
+            raise RuntimeError("push_frames needs an upsample network the native upsampler covers (engine.upsampler_struct)")
+        self._frames = frames if self._frames is None else torch.cat([self._frames, frames], dim=-1)
+        return self._frames_chunk(final=False)
+
+    @torch.no_grad()
+    def finish(self):
+        """The samples left once no further frame follows, up to the upsampled length of all frames pushed."""
+        if self._m.upsample_net is None or self._frames is None:
+            self._finished = True
+            return self._empty()
+        out = self._frames_chunk(final=True)
+        self._finished = True
+        return out
+
+    def _frames_chunk(self, final):
+        n = self._frames.size(-1)
+        t = self.t
+        _, _, ready = self._eng.upsample_cone(n, final)
+        if ready <= t:
+            return self._empty()
+        f_lo, f_hi, _ = self._eng.upsample_cone(n, final, t, ready)
+        return self._chunk(ready - t, c_frames=self._frames[:, :, f_lo:f_hi], frame_offset=f_lo, frames_total=n,
+                           final=final)
