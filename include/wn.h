@@ -273,6 +273,25 @@ int32_t wn_pack_cta(const wn_config* cfg, int32_t batch, int32_t num_sms, int64_
 int32_t wn_plan_passes(const wn_config* cfg, int32_t batch, int32_t num_sms, int64_t smem_per_cta,
                        int32_t* plan_words, int32_t max_plan_words, void* passes, int32_t max_passes);
 
+/* ---- Teacher-forced scoring (added in ABI 3 without changing WN_ABI_VERSION or any struct: wn_struct_sizes still
+ * reports 7 structs; a binding detects these two entry points by their presence in the library).
+ *
+ * Teacher-forced batch forward (reference WaveNet.forward): writes params_out (B,O,T), the head output a fully
+ * teacher-forced wn_generate would write, computed in parallel over time (dense 3xTF32 GEMMs, csrc/wn_dense.cuh).
+ * Reads B, T, T_test (== T) and exactly one of test_scalar / test_index / test_dense; c or c_frames (through the loaded
+ * upsampler) and g as wn_generate does; flags (WN_FLAG_SOFTMAX only: a softmax over O); params_out; stream.  Refused
+ * with WN_ERR_INVALID: any noise_* or out_* pointer, initial / initial_rows / initial_dense, T_test != T.
+ * initial_index is not read.  Returns after the launches are enqueued; wn_sync(handle) waits for them.  The activation
+ * scratch grows as needed (WN_ERR_NOMEM says how many bytes were needed). */
+int32_t wn_forward(void* handle, const wn_generate_args* a);
+/* Per-sample negative log-likelihood of y_target (B,T) [MoL, Gauss] or class_target (B,T) [softmax] under the
+ * head outputs y_bot (B,O,T); DEVICE pointers; out (B,T).  The reference's discretized_mix_logistic_loss
+ * (mixture.py:26-106, num_classes and log_scale_min as given), mix_gaussian_loss (mixture.py:161-218) and the
+ * cross-entropy of the softmax head (train.py:346-362), each with reduce=False.  num_classes >= 2 (read by MoL only);
+ * a class outside [0,O) gives NaN.  The arguments are checked before the device is touched. */
+int32_t wn_nll(const float* y_bot, int32_t head_kind, int32_t B, int32_t O, int32_t T, const float* y_target,
+               const int32_t* class_target, int32_t num_classes, float log_scale_min, float* out_bt, void* stream);
+
 /* Stand-alone samplers over a (B,O,T) head-output tensor (DEVICE), the reference's
  * mixture.py entry points; noise is REPLAY layout with T as given. out: (B,T). */
 int32_t wn_sample_mol(const float* y_bot, int32_t B, int32_t O, int32_t T,

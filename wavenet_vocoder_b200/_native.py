@@ -16,7 +16,8 @@ ROOT = os.path.dirname(HERE)
 LIB_PATH = os.path.join(HERE, "libwn.so")
 SOURCES = [os.path.join(HERE, "csrc", "wn_host.cu")]
 HEADERS = [os.path.join(HERE, "csrc", f) for f in ("wn_plan.h", "wn_kernel.cuh", "wn7_plan.h", "wn7_kernel.cuh",
-                                                     "wn7_host.cuh", "wn_aux.cuh")] + [os.path.join(ROOT, "include", "wn.h")]
+                                                     "wn7_host.cuh", "wn_aux.cuh",
+                                                     "wn_dense.cuh")] + [os.path.join(ROOT, "include", "wn.h")]
 
 WN_ABI_VERSION = 3
 WN_INPUT_SCALAR, WN_INPUT_ONEHOT = 0, 1
@@ -147,7 +148,11 @@ EXPORTS = ["wn_abi_version", "wn_struct_sizes", "wn_last_error", "wn_create", "w
            "wn_generate", "wn_sync", "wn_generate_host", "wn_get_plan", "wn_plan_only",
            "wn_pack_cta", "wn_plan_passes", "wn_load_upsampler", "wn_upsample", "wn_decode", "wn_sample_mol", "wn_sample_gauss",
            "wn_stream_open", "wn_stream_generate", "wn_stream_position", "wn_stream_close", "wn_upsample_cone",
-           "wn_decode_stream"]
+           "wn_decode_stream", "wn_forward", "wn_nll"]
+
+
+# entry points an older build of ABI 3 may lack (bound when present)
+OPTIONAL_EXPORTS = ("wn_struct_sizes", "wn_forward", "wn_nll")
 
 
 def nvcc_command(out=LIB_PATH):
@@ -234,8 +239,12 @@ def _bind(L):
     L.wn_upsample_cone.argtypes = [C.POINTER(wn_upsampler), C.c_int64, C.c_int32, C.c_int64, C.c_int64, _i64p, _i64p,
                                    _i64p]
     L.wn_decode_stream.argtypes = L.wn_decode.argtypes[:-1] + [C.c_void_p, C.c_void_p]
+    if hasattr(L, "wn_forward"):           # added to ABI 3 without a version bump: detected by presence
+        L.wn_forward.argtypes = [C.c_void_p, C.POINTER(wn_generate_args)]
+        L.wn_nll.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32,
+                             C.c_float, C.c_void_p, C.c_void_p]
     for n in EXPORTS:
-        if n == "wn_struct_sizes" and not hasattr(L, n):
+        if n in OPTIONAL_EXPORTS and not hasattr(L, n):
             continue                       # an older build of the same ABI (A/B experiments through WN_LIB_PATH)
         fn = getattr(L, n)
         if n != "wn_last_error":

@@ -17,6 +17,7 @@
 #include "wn7_plan.h"
 #include "wn7_kernel.cuh"
 #include "wn_aux.cuh"
+#include "wn_dense.cuh"
 
 // ------------------------------------------------------------------------------------------
 // errors
@@ -472,6 +473,8 @@ struct WnHandle {
     size_t l2_persist_bytes = 0, l2_window_max = 0;   // persisting-L2 carve-out
     int l2_mode = 0;                                  // WN_L2_PERSIST: 1 = packed weights, 2 = exchange buffer
     size_t wpack_bytes = 0;
+    float* d_dense = nullptr;  size_t dense_bytes = 0;    // unfolded fp32 matrices of the batch forward (DenseLayout)
+    float* d_fwd = nullptr;    size_t fwd_bytes = 0;      // wn_forward activation scratch
 };
 
 template <typename T>
@@ -876,6 +879,103 @@ static int32_t launch_chunk7(WnHandle* h, const wn_generate_args* a, int b0, int
 }
 
 // ------------------------------------------------------------------------------------------
+// teacher-forced batch forward (wn_forward): csrc/wn_dense.cuh
+// ------------------------------------------------------------------------------------------
+// The dense image holds the fp32 matrices as they arrive in wn_weights (row-major M x K), not folded: per layer
+// [conv_w | cond_w] (G x kw*R+C), conv_b (G), [out_w ; skip_w] (R+S x G/2), [out_b ; skip_b] (R+S); then last_a_w,
+// last_a_b, last_b_w, last_b_b.  Every piece starts at a multiple of 4 floats.
+struct DenseLayout {
+    size_t gate_w, gate_b, os_w, os_b, per_layer;   // offsets within one layer
+    size_t la_w, la_b, lb_w, lb_b, total;            // offsets of the head, total floats
+};
+
+static DenseLayout dense_layout(const wn_config& c) {
+    auto al = [](size_t v) { return (v + 3) / 4 * 4; };
+    const size_t R = c.residual_channels, G = c.gate_channels, G2 = G / 2, S = c.skip_channels, O = c.out_channels;
+    const size_t Kg = (size_t)c.kernel_size * R + c.cin_channels;
+    DenseLayout d;
+    d.gate_w = 0;
+    d.gate_b = al(G * Kg);
+    d.os_w = d.gate_b + al(G);
+    d.os_b = d.os_w + al((R + S) * G2);
+    d.per_layer = d.os_b + al(R + S);
+    d.la_w = (size_t)c.layers * d.per_layer;
+    d.la_b = d.la_w + al(S * S);
+    d.lb_w = d.la_b + al(S);
+    d.lb_b = d.lb_w + al(O * S);
+    d.total = d.lb_b + al(O);
+    return d;
+}
+
+static void pack_dense(const wn_config& c, const wn_weights& w, std::vector<float>& img) {
+    const DenseLayout d = dense_layout(c);
+    const size_t R = c.residual_channels, G = c.gate_channels, G2 = G / 2, S = c.skip_channels, O = c.out_channels;
+    const size_t kwR = (size_t)c.kernel_size * R, Cc = c.cin_channels, Kg = kwR + Cc;
+    img.assign(d.total, 0.f);
+    auto put = [&](size_t off, const float* src, size_t n) { memcpy(img.data() + off, src, n * sizeof(float)); };
+    for (int l = 0; l < c.layers; ++l) {
+        const wn_layer_weights& lw = w.layers[l];
+        const size_t base = (size_t)l * d.per_layer;
+        for (size_t row = 0; row < G; ++row) {
+            put(base + d.gate_w + row * Kg, lw.conv_w + row * kwR, kwR);
+            if (Cc) put(base + d.gate_w + row * Kg + kwR, lw.cond_w + row * Cc, Cc);
+        }
+        put(base + d.gate_b, lw.conv_b, G);
+        put(base + d.os_w, lw.out_w, R * G2);
+        put(base + d.os_w + R * G2, lw.skip_w, S * G2);
+        put(base + d.os_b, lw.out_b, R);
+        put(base + d.os_b + R, lw.skip_b, S);
+    }
+    put(d.la_w, w.last_a_w, S * S);
+    put(d.la_b, w.last_a_b, S);
+    put(d.lb_w, w.last_b_w, O * S);
+    put(d.lb_b, w.last_b_b, O);
+}
+
+// the conditioning inputs of a call (c or c_frames, g); window_frames: c_frames is a window of the utterance (a stream
+// chunk, checked by the caller), not all of it
+static int32_t validate_cond(const WnHandle* h, const wn_generate_args* a, bool window_frames) {
+    const wn_config& c = h->cfg;
+    if (a->c && a->c_frames) return fail(WN_ERR_INVALID, "give either c (sample rate) or c_frames, not both");
+    if (c.cin_channels > 0 && !a->c && !a->c_frames) return fail(WN_ERR_INVALID, "c is required (cin_channels > 0), cf. train.py:82-87");
+    if (c.cin_channels == 0 && (a->c || a->c_frames)) return fail(WN_ERR_INVALID, "c given but the model has no local conditioning");
+    if (a->c_frames && window_frames) {
+        if (!h->have_ups) return fail(WN_ERR_STATE, "c_frames given but no upsampler was loaded (wn_load_upsampler)");
+    } else if (a->c_frames) {
+        if (!h->have_ups) return fail(WN_ERR_STATE, "c_frames given but no upsampler was loaded (wn_load_upsampler)");
+        const long long Fo = (long long)a->n_frames - (h->ups_ks > 0 ? h->ups_ks - 1 : 0);
+        if (Fo < 1 || Fo * h->ups_total - 2LL * h->ups.indent != (long long)a->T)
+            return fail(WN_ERR_INVALID, "upsampled conditioning length != T (wavenet.py:276)");
+    }
+    if (c.gin_channels == 0 && a->g) return fail(WN_ERR_INVALID, "g given but the model has no global conditioning");
+    return WN_OK;
+}
+
+static int32_t validate_forward(const WnHandle* h, const wn_generate_args* a) {
+    const wn_config& c = h->cfg;
+    if (!a) return fail(WN_ERR_INVALID, "null args");
+    if (a->B < 1 || a->T < 1) return fail(WN_ERR_INVALID, "B and T must be >= 1");
+    if (a->T_test != a->T) return fail(WN_ERR_INVALID, "wn_forward: T_test must equal T (every step is teacher forced)");
+    const int nx = (a->test_scalar != nullptr) + (a->test_index != nullptr) + (a->test_dense != nullptr);
+    if (nx != 1) return fail(WN_ERR_INVALID, "wn_forward: give exactly one of test_scalar, test_index, test_dense");
+    if (c.input_kind == WN_INPUT_SCALAR && !a->test_scalar)
+        return fail(WN_ERR_INVALID, "wn_forward: a scalar-input model takes test_scalar");
+    if (c.input_kind == WN_INPUT_ONEHOT && a->test_scalar)
+        return fail(WN_ERR_INVALID, "wn_forward: a one-hot-input model takes test_index or test_dense");
+    if (a->noise_u1 || a->noise_u2 || a->noise_z || a->noise_e)
+        return fail(WN_ERR_INVALID, "wn_forward draws no noise: noise_u1, noise_u2, noise_z and noise_e must be NULL");
+    if (a->out_scalar || a->out_index || a->out_dense)
+        return fail(WN_ERR_INVALID, "wn_forward writes params_out only: out_scalar, out_index and out_dense must be NULL");
+    if (a->initial || a->initial_rows || a->initial_dense)
+        return fail(WN_ERR_INVALID, "wn_forward: initial, initial_rows and initial_dense must be NULL (every step is "
+                                    "teacher forced)");
+    if (!a->params_out) return fail(WN_ERR_INVALID, "wn_forward: params_out required");
+    if (a->flags & ~WN_FLAG_SOFTMAX) return fail(WN_ERR_INVALID, "wn_forward: only WN_FLAG_SOFTMAX applies");
+    if (c.gin_channels > 0 && !a->g) return fail(WN_ERR_INVALID, "g is required (gin_channels > 0)");
+    return validate_cond(h, a, false);
+}
+
+// ------------------------------------------------------------------------------------------
 // C ABI
 // ------------------------------------------------------------------------------------------
 extern "C" {
@@ -1044,6 +1144,7 @@ int32_t wn_destroy(void* handle) {
     cudaFree(h->d_ringtab); cudaFree(h->d_err); cudaFree(h->d_xbuf); cudaFree(h->d_ring); cudaFree(h->d_gbias);
     cudaFree(h->d_scratch);
     cudaFree(h->d_prof);
+    cudaFree(h->d_dense); cudaFree(h->d_fwd);
     delete h;
     return WN_OK;
 }
@@ -1123,6 +1224,12 @@ int32_t wn_load_weights(void* handle, const wn_weights* w) {
     CUDA_TRY(cudaMalloc((void**)&h->d_ringtab, std::max<size_t>(16, h->ringtab.size() * sizeof(int))));
     if (!h->ringtab.empty())
         CUDA_TRY(cudaMemcpy(h->d_ringtab, h->ringtab.data(), h->ringtab.size() * sizeof(int), cudaMemcpyHostToDevice));
+    {   // the unfolded matrices wn_forward reads: uploaded with the packed image, so neither path can see stale weights
+        std::vector<float> dense;
+        pack_dense(c, *w, dense);
+        if ((rc = upload(&h->d_dense, dense))) return rc;
+        h->dense_bytes = dense.size() * sizeof(float);
+    }
     h->have_weights = true;
     return WN_OK;
 }
@@ -1133,18 +1240,8 @@ static int32_t validate_args(const WnHandle* h, const wn_generate_args* a, bool 
     if (!a) return fail(WN_ERR_INVALID, "null args");
     if (a->B < 1 || a->T < 1) return fail(WN_ERR_INVALID, "B and T must be >= 1");
     if ((long long)a->T * (c.layers + 3LL) >= 0xFFFFFFF0LL) return fail(WN_ERR_INVALID, "T too large for 32-bit tags");
-    if (a->c && a->c_frames) return fail(WN_ERR_INVALID, "give either c (sample rate) or c_frames, not both");
-    if (c.cin_channels > 0 && !a->c && !a->c_frames) return fail(WN_ERR_INVALID, "c is required (cin_channels > 0), cf. train.py:82-87");
-    if (c.cin_channels == 0 && (a->c || a->c_frames)) return fail(WN_ERR_INVALID, "c given but the model has no local conditioning");
-    if (a->c_frames && window_frames) {
-        if (!h->have_ups) return fail(WN_ERR_STATE, "c_frames given but no upsampler was loaded (wn_load_upsampler)");
-    } else if (a->c_frames) {
-        if (!h->have_ups) return fail(WN_ERR_STATE, "c_frames given but no upsampler was loaded (wn_load_upsampler)");
-        const long long Fo = (long long)a->n_frames - (h->ups_ks > 0 ? h->ups_ks - 1 : 0);
-        if (Fo < 1 || Fo * h->ups_total - 2LL * h->ups.indent != (long long)a->T)
-            return fail(WN_ERR_INVALID, "upsampled conditioning length != T (wavenet.py:276)");
-    }
-    if (c.gin_channels == 0 && a->g) return fail(WN_ERR_INVALID, "g given but the model has no global conditioning");
+    int32_t rc = validate_cond(h, a, window_frames);
+    if (rc) return rc;
     if (a->T_test < 0 || a->T_test > a->T) return fail(WN_ERR_INVALID, "T_test must be in [0,T] (wavenet.py:258)");
     if (c.input_kind == WN_INPUT_SCALAR) {
         if (!a->out_scalar) return fail(WN_ERR_INVALID, "out_scalar required");
@@ -1652,6 +1749,174 @@ int32_t wn_sample_gauss(const float* y_bot, int32_t B, int32_t O, int32_t T, con
     if (O > 3 && !u1_tbk) return fail(WN_ERR_INVALID, "u1 required for a mixture");
     const int n = B * T;
     wn::wn_sample_kernel<<<(n + 255) / 256, 256, 0, (cudaStream_t)stream>>>(y_bot, B, O, T, u1_tbk, z_tb, out_bt, 1);
+    CUDA_TRY(cudaGetLastError());
+    return WN_OK;
+}
+
+int32_t wn_forward(void* handle, const wn_generate_args* a) {
+    WnHandle* h = (WnHandle*)handle;
+    if (!h) return fail(WN_ERR_INVALID, "null handle");
+    if (!h->have_weights || !h->d_dense) return fail(WN_ERR_STATE, "wn_forward before wn_load_weights");
+    int32_t rc = validate_forward(h, a);
+    if (rc) return rc;
+    DeviceGuard guard(h->cfg.device);
+    const wn_config& c = h->cfg;
+    cudaStream_t st = (cudaStream_t)a->stream;
+    const int B = a->B, T = a->T, L = c.layers, R = c.residual_channels, G = c.gate_channels, G2 = G / 2;
+    const int S = c.skip_channels, O = c.out_channels, kw = c.kernel_size, Cc = c.cin_channels;
+    const int per_stack = L / c.stacks;
+    // scratch: X (B,R,T) | Y, then the head's hidden layer (B,max(G/2,S),T) | skip sum (B,S,T) | c^T (B,C,T) |
+    // a dense one-hot input transposed (B,O,T)
+    auto al = [](size_t v) { return (v + 63) / 64 * 64; };
+    const size_t BT = (size_t)B * T;
+    const size_t oY = al(BT * R), oS = oY + al(BT * std::max(G2, S)), oC = oS + al(BT * S), oD = oC + al(BT * Cc);
+    const size_t need = (oD + (a->test_dense ? al(BT * O) : 0) + 64) * sizeof(float);
+    if (ensure(&h->d_fwd, &h->fwd_bytes, need)) {
+        cudaGetLastError();
+        return fail(WN_ERR_NOMEM, "wn_forward: cannot allocate " + std::to_string(need) + " bytes of activation scratch");
+    }
+    float *X = h->d_fwd, *Y = h->d_fwd + oY, *skip = h->d_fwd + oS, *cT = h->d_fwd + oC, *xdT = h->d_fwd + oD;
+    int64_t launches = 0;
+    const float* cond = a->c;
+    if (a->c_frames) {
+        rc = run_upsampler(h, a->c_frames, B, a->n_frames, T, st);
+        if (rc) return rc;
+        cond = h->d_cup;
+    }
+    if (Cc > 0) {
+        wnd::transpose_tc_kernel<<<dim3((T + 31) / 32, (Cc + 31) / 32, B), dim3(32, 8), 0, st>>>(cond, cT, T, Cc);
+        CUDA_TRY(cudaGetLastError());
+        ++launches;
+    }
+    const float* gb = nullptr;
+    if (c.gin_channels > 0) {         // W_g . g once per call, as the synthesis path does
+        rc = ensure(&h->d_gbias, &h->gbias_bytes, (size_t)B * L * G * sizeof(float));
+        if (rc) return rc;
+        wn::wn_gbias_kernel<<<dim3(L, B), 128, 0, st>>>(h->d_wg, a->g, h->d_gbias, L, G, c.gin_channels);
+        CUDA_TRY(cudaGetLastError());
+        ++launches;
+        gb = h->d_gbias;
+    }
+    if (a->test_dense) {
+        wnd::transpose_tc_kernel<<<dim3((T + 31) / 32, (O + 31) / 32, B), dim3(32, 8), 0, st>>>(a->test_dense, xdT, T, O);
+        CUDA_TRY(cudaGetLastError());
+        ++launches;
+    }
+    {
+        const long long n = (long long)BT * R;
+        const int blocks = (int)std::min<long long>((n + 255) / 256, 1 << 16);
+        wnd::first_conv_kernel<<<blocks, 256, 0, st>>>(a->test_scalar, a->test_index, a->test_dense ? xdT : nullptr,
+                                                       h->d_first_w, h->d_first_b, X, B, R, O, T);
+        CUDA_TRY(cudaGetLastError());
+        ++launches;
+    }
+    const DenseLayout d = dense_layout(c);
+    for (int l = 0; l < L; ++l) {
+        const float* lw = h->d_dense + (size_t)l * d.per_layer;
+        wnd::DenseGemm p;
+        memset(&p, 0, sizeof(p));
+        p.A = lw + d.gate_w;
+        p.M = G;
+        p.K = kw * R + Cc;
+        p.T = T;
+        p.X = X;
+        p.cT = Cc > 0 ? cT : nullptr;
+        p.R = R;
+        p.kw = kw;
+        p.dil = 1 << (l % per_stack);
+        p.Cc = Cc;
+        p.kwR = kw * R;
+        p.bias = lw + d.gate_b;
+        p.gbias = gb ? gb + (size_t)l * G : nullptr;
+        p.gstride = (long long)L * G;
+        p.G2 = G2;
+        p.out = Y;
+        CUDA_TRY((wnd::launch_dense_gemm<wnd::B_GATE, wnd::EPI_GATE>(p, B, st)));
+        wnd::DenseGemm q;
+        memset(&q, 0, sizeof(q));
+        q.A = lw + d.os_w;
+        q.M = R + S;
+        q.K = G2;
+        q.T = T;
+        q.Bsrc = Y;
+        q.R = R;
+        q.bias = lw + d.os_b;
+        q.out = X;
+        q.out2 = skip;
+        q.first = l == 0;
+        CUDA_TRY((wnd::launch_dense_gemm<wnd::B_PLAIN, wnd::EPI_RESSKIP>(q, B, st)));
+        launches += 2;
+    }
+    {   // relu(skip * sqrt(1/L)) -> last_a -> relu -> last_b (wavenet.py:207-210)
+        wnd::DenseGemm p;
+        memset(&p, 0, sizeof(p));
+        p.A = h->d_dense + d.la_w;
+        p.M = S;
+        p.K = S;
+        p.T = T;
+        p.Bsrc = skip;
+        p.brelu = 1;
+        p.bscale = (float)std::sqrt(1.0 / L);
+        p.bias = h->d_dense + d.la_b;
+        p.out = Y;
+        CUDA_TRY((wnd::launch_dense_gemm<wnd::B_PLAIN, wnd::EPI_RELU_BIAS>(p, B, st)));
+        wnd::DenseGemm q;
+        memset(&q, 0, sizeof(q));
+        q.A = h->d_dense + d.lb_w;
+        q.M = O;
+        q.K = S;
+        q.T = T;
+        q.Bsrc = Y;
+        q.bias = h->d_dense + d.lb_b;
+        q.out = a->params_out;
+        CUDA_TRY((wnd::launch_dense_gemm<wnd::B_PLAIN, wnd::EPI_BIAS>(q, B, st)));
+        launches += 2;
+    }
+    if (a->flags & WN_FLAG_SOFTMAX) {
+        const int blocks = (int)std::min<long long>(((long long)BT + 255) / 256, 1 << 16);
+        wnd::col_softmax_kernel<<<blocks, 256, 0, st>>>(a->params_out, B, O, T);
+        CUDA_TRY(cudaGetLastError());
+        ++launches;
+    }
+    h->launches += launches;
+    h->last_stream = st;
+    h->pending = true;
+    return WN_OK;
+}
+
+int32_t wn_nll(const float* y_bot, int32_t head_kind, int32_t B, int32_t O, int32_t T, const float* y_target,
+               const int32_t* class_target, int32_t num_classes, float log_scale_min, float* out_bt, void* stream) {
+    if (!y_bot || !out_bt) return fail(WN_ERR_INVALID, "wn_nll: null argument");
+    if (B < 1 || T < 1 || O < 1) return fail(WN_ERR_INVALID, "wn_nll: B, O and T must be >= 1");
+    if (y_target && class_target) return fail(WN_ERR_INVALID, "wn_nll: give y_target or class_target, not both");
+    if (!y_target && !class_target) return fail(WN_ERR_INVALID, "wn_nll: a target is required");
+    if (num_classes < 2) return fail(WN_ERR_INVALID, "wn_nll: num_classes must be >= 2");
+    if (head_kind == WN_HEAD_MOL) {
+        if (O % 3 != 0) return fail(WN_ERR_INVALID, "wn_nll: a MoL head has 3K channels (mixture.py:44)");
+    } else if (head_kind == WN_HEAD_GAUSS) {
+        if (O != 2 && O % 3 != 0) return fail(WN_ERR_INVALID, "wn_nll: a Gaussian head has 2 or 3K channels (mixture.py:176-181)");
+    } else if (head_kind != WN_HEAD_SOFTMAX) {
+        return fail(WN_ERR_INVALID, "wn_nll: bad head_kind");
+    }
+    if (head_kind == WN_HEAD_SOFTMAX ? !class_target : !y_target)
+        return fail(WN_ERR_INVALID, head_kind == WN_HEAD_SOFTMAX ? "wn_nll: a softmax head takes class_target"
+                                                                  : "wn_nll: a MoL or Gaussian head takes y_target");
+    wnd::NllArgs na;
+    memset(&na, 0, sizeof(na));
+    na.y = y_bot;
+    na.yt = y_target;
+    na.ct = class_target;
+    na.out = out_bt;
+    na.head = head_kind == WN_HEAD_MOL ? wnd::NLL_MOL : head_kind == WN_HEAD_GAUSS ? wnd::NLL_GAUSS : wnd::NLL_SOFTMAX;
+    na.B = B;
+    na.O = O;
+    na.T = T;
+    na.log_scale_min = log_scale_min;
+    na.half_bin = (float)(1.0 / (num_classes - 1));
+    na.log_half_nc = (float)std::log((num_classes - 1) / 2.0);
+    const long long n = (long long)B * T;
+    const int blocks = (int)std::min<long long>((n + 255) / 256, 1 << 16);
+    wnd::nll_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(na);
     CUDA_TRY(cudaGetLastError());
     return WN_OK;
 }

@@ -160,6 +160,30 @@ def upsample_cone(u, n_frames, final, t_lo=0, t_hi=0):
     return f_lo.value, f_hi.value, n_ready.value
 
 
+def nll(head: torch.Tensor, head_kind: int, target: torch.Tensor, num_classes: int = 65536,
+        log_scale_min: float = -16.0) -> torch.Tensor:
+    """wn_nll: per-sample negative log-likelihood (B,T) of ``target`` under head outputs ``head`` (B,O,T) on a CUDA
+    device -- the reference's discretized_mix_logistic_loss / mix_gaussian_loss / cross-entropy with reduce=False.
+    ``target``: (B,T) samples in [-1,1] for a MoL or Gaussian head, (B,T) class ids for a softmax head."""
+    if head.device.type != "cuda" or head.dim() != 3:
+        raise ValueError("head must be a (B,O,T) CUDA tensor")
+    B, O, T = head.shape
+    y = head.float().contiguous()
+    if tuple(target.shape) != (B, T):
+        raise ValueError("target must be (B,T) = (%d,%d), got %s" % (B, T, tuple(target.shape)))
+    yt = ct = None
+    if head_kind == N.WN_HEAD_SOFTMAX:
+        ct = target.to(device=head.device, dtype=torch.int32).contiguous()
+    else:
+        yt = target.to(device=head.device, dtype=torch.float32).contiguous()
+    out = torch.empty(B, T, device=head.device, dtype=torch.float32)
+    stream = torch.cuda.current_stream(head.device)
+    N.check(N.lib().wn_nll(y.data_ptr(), int(head_kind), B, O, T, None if yt is None else yt.data_ptr(),
+                           None if ct is None else ct.data_ptr(), int(num_classes), float(log_scale_min),
+                           out.data_ptr(), stream.cuda_stream))
+    return out
+
+
 class SynthesisStream:
     """One utterance (or one batch tile of them) made chunk by chunk; the state between chunks stays on the device
     (wn_stream_* of include/wn.h).  Chunks are bit-identical to the same samples of one ``generate`` call."""
@@ -468,6 +492,56 @@ class SynthesisEngine:
         if sync:
             self.sync()
         return out, params
+
+    # ------------------------------------------------------------------ teacher-forced scoring
+    def forward(self, *, test_scalar: Optional[torch.Tensor] = None, test_index: Optional[torch.Tensor] = None,
+                test_dense: Optional[torch.Tensor] = None, c: Optional[torch.Tensor] = None,
+                c_frames: Optional[torch.Tensor] = None, g: Optional[torch.Tensor] = None, softmax=False, sync=True):
+        """Teacher-forced batch forward (wn_forward): the head outputs (B,O,T) of every step, computed in parallel over
+        time.  The input is exactly one of test_scalar (B,T), test_index (B,T) class ids or test_dense (B,T,O); c, c_frames
+        and g as in ``generate``; ``softmax`` applies a softmax over O."""
+        given = [t for t in (test_scalar, test_index, test_dense) if t is not None]
+        if len(given) != 1:
+            raise ValueError("give exactly one of test_scalar, test_index, test_dense")
+        dev, O = self.device, self.out_channels
+        B, T = int(given[0].size(0)), int(given[0].size(1))
+        a = N.wn_generate_args()
+        a.B, a.T, a.T_test = B, T, T
+        hold = []
+
+        def dptr(t, dtype=torch.float32, shape=None):
+            if t is None:
+                return None
+            t = t.to(device=dev, dtype=dtype).contiguous()
+            if shape is not None and tuple(t.shape) != tuple(shape):
+                raise ValueError("expected shape %s, got %s" % (tuple(shape), tuple(t.shape)))
+            hold.append(t)
+            return t.data_ptr()
+
+        a.test_scalar = dptr(test_scalar, shape=(B, T))
+        a.test_index = dptr(test_index, torch.int32, shape=(B, T))
+        a.test_dense = dptr(test_dense, shape=(B, T, O))
+        a.c = dptr(c, shape=(B, T, self.cin) if c is not None else None)
+        if c_frames is not None:
+            a.c_frames = dptr(c_frames, shape=(B, self.cin, c_frames.size(-1)))
+            a.n_frames = int(c_frames.size(-1))
+        a.g = dptr(g, shape=(B, self.gin) if g is not None else None)
+        a.initial_index = -1
+        a.flags = N.WN_FLAG_SOFTMAX if softmax else 0
+        params = torch.empty(B, O, T, device=dev, dtype=torch.float32)
+        a.params_out = params.data_ptr()
+        a.stream = torch.cuda.current_stream(dev).cuda_stream
+        N.check(N.lib().wn_forward(self._h, C.byref(a)))
+        self._keep = hold
+        if sync:
+            self.sync()
+        return params
+
+    def nll(self, head: torch.Tensor, target: torch.Tensor, num_classes: int = 65536,
+            log_scale_min: float = -16.0) -> torch.Tensor:
+        """Per-sample negative log-likelihood (B,T) of ``target`` under head outputs (B,O,T) of this model's output
+        head (wn_nll); see ``nll``."""
+        return nll(head, self.head, target, num_classes=num_classes, log_scale_min=log_scale_min)
 
     # ------------------------------------------------------------------ streaming
     def open_stream(self, **kw) -> SynthesisStream:

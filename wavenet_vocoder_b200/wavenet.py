@@ -337,6 +337,105 @@ class WaveNet(nn.Module):
             y = out
         return (y, params) if return_params else y
 
+    # ------------------------------------------------------------------ teacher-forced scoring on the device
+    @torch.no_grad()
+    def forward_native(self, x, c=None, g=None, softmax=False):
+        """``forward(x, c, g, softmax)`` on the native engine (csrc/wn_dense.cuh): the same arguments and return value
+        (B,out_channels,T), in eval mode and without autograd, every step computed in parallel in fp32-accurate
+        (3xTF32) arithmetic.  ``c``: conditioning frames (upsampled on the device when the native upsampler covers the
+        network, else by the PyTorch network in IEEE fp32) or sample-rate (B,C,T) / (B,T,C); ``g``: speaker ids or
+        (B,gin[,1]) features, one vector per utterance."""
+        if self.training:
+            raise RuntimeError("forward_native only supports eval mode (use forward() for training)")
+        if next(self.parameters()).device.type != "cuda":
+            raise RuntimeError("WaveNet.forward_native runs on a CUDA device only (no CPU fallback); move the model "
+                               "with .to('cuda') or use forward()")
+        eng = self._get_engine()
+        dev = eng.device
+        O = self.out_channels
+        x = x.to(dev)
+        B, _, T = x.size()
+        test_scalar = test_index = test_dense = None
+        if self.scalar_input:
+            if x.size(1) != 1:
+                raise ValueError("a scalar-input model takes x of shape (B,1,T)")
+            test_scalar = x[:, 0, :].float().contiguous()
+        else:
+            if x.size(1) != O:
+                raise ValueError("a one-hot-input model takes x of shape (B,%d,T)" % O)
+            xt = x.float().transpose(1, 2).contiguous()                              # (B,T,O)
+            idx = xt.argmax(-1)
+            if torch.equal(torch.zeros_like(xt).scatter_(-1, idx.unsqueeze(-1), 1.0), xt):
+                test_index = idx.to(torch.int32)
+            else:
+                test_dense = xt
+        g_vec = None
+        if g is not None:
+            g = g.to(dev)
+            if self.embed_speakers is not None:
+                g_vec = self.embed_speakers(g.view(B, -1).long())[:, 0, :]        # wavenet.py:187-189
+            else:
+                if g.dim() == 3 and g.size(-1) != 1:
+                    raise ValueError("forward_native takes one global-conditioning vector per utterance")
+                g_vec = g.reshape(B, -1).float()
+        c_frames = None
+        if c is not None:
+            c = c.to(dev).float()
+            if self.upsample_net is not None and self._native_upsample and \
+                    os.environ.get("WN_TORCH_UPSAMPLE", "0") != "1":
+                if c.dim() != 3 or c.size(1) != self.cin_channels or eng.upsampled_length(c.size(-1)) != T:
+                    raise ValueError("conditioning frames %s do not upsample to T=%d" % (tuple(c.shape), T))
+                c_frames, c = c.contiguous(), None
+            else:
+                if self.upsample_net is not None:
+                    c = _upsample_fp32(self.upsample_net, c)
+                if c.dim() == 3 and c.size(1) == self.cin_channels and c.size(2) == T:
+                    c = c.transpose(1, 2)
+                if c.dim() != 3 or c.size(0) != B or c.size(1) != T or c.size(2) != self.cin_channels:
+                    raise ValueError("conditioning of shape %s does not match x (B=%d, T=%d)" % (tuple(c.shape), B, T))
+                c = c.contiguous()
+        return eng.forward(test_scalar=test_scalar, test_index=test_index, test_dense=test_dense, c=c,
+                           c_frames=c_frames, g=g_vec, softmax=bool(softmax))
+
+    @torch.no_grad()
+    def nll(self, x, c=None, g=None, y=None, lengths=None, num_classes=65536, log_scale_min=-16.0, reduce=True):
+        """Teacher-forced negative log-likelihood, as the reference's training criterion computes it
+        (train.py:727-748): head outputs ``forward_native(x, c, g)[:, :, :-1]`` against targets ``y[:, 1:]``.
+        ``y`` defaults to x itself: the samples for scalar input, the class ids for exactly one-hot input (otherwise
+        pass ``y``, (B,T) or (B,T,1)).  ``reduce``: the mean over the mask ``sequence_mask(lengths)[:, 1:]`` (all
+        samples without ``lengths``); otherwise the per-sample losses (B,T-1).  The defaults of ``num_classes`` and
+        ``log_scale_min`` are the reference's hparams (quantize_channels, log_scale_min)."""
+        head = self.forward_native(x, c=c, g=g, softmax=False)
+        B, _, T = head.shape
+        if T < 2:
+            raise ValueError("nll needs T >= 2 (the head at step t scores the sample at t+1)")
+        dev = head.device
+        if y is None:
+            if self.scalar_input:
+                y = x[:, 0, :]
+            else:
+                xt = x.to(dev).float()
+                idx = xt.argmax(1)
+                if not torch.equal(torch.zeros_like(xt).scatter_(1, idx.unsqueeze(1), 1.0), xt):
+                    raise ValueError("x is not exactly one-hot: pass the target classes as y")
+                y = idx
+        y = y.to(dev)
+        if y.dim() == 3:
+            y = y[:, :, 0] if y.size(-1) == 1 else y[:, 0, :]
+        if tuple(y.shape) != (B, T):
+            raise ValueError("y must be (B,T) = (%d,%d), got %s" % (B, T, tuple(y.shape)))
+        losses = self._get_engine().nll(head[:, :, :-1].contiguous(), y[:, 1:].contiguous(), num_classes=num_classes,
+                                        log_scale_min=log_scale_min)
+        if not reduce:
+            return losses
+        if lengths is None:
+            return losses.mean()
+        lengths = torch.as_tensor(lengths, device=dev).long().view(-1)
+        if lengths.numel() != B or int(lengths.max()) > T or int(lengths.min()) < 0:
+            raise ValueError("lengths must be B values in [0, T=%d]" % T)
+        mask = (torch.arange(T, device=dev).unsqueeze(0) < lengths.unsqueeze(1))[:, 1:].float()   # train.py:728-729
+        return (losses * mask).sum() / mask.sum()
+
     # ------------------------------------------------------------------ streaming
     @torch.no_grad()
     def open_stream(self, B=1, g=None, initial_input=None, seed=None, noise=None, softmax=True, quantize=True,
