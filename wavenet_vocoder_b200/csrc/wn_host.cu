@@ -472,6 +472,8 @@ struct WnHandle {
     bool attr_set[40] = {};       // [20, 40): the stream instantiations
     size_t l2_persist_bytes = 0, l2_window_max = 0;   // persisting-L2 carve-out
     int l2_mode = 0;                                  // WN_L2_PERSIST: 1 = packed weights, 2 = exchange buffer
+    size_t l2_bytes = 0, l2_carve_bytes = 0;          // L2 size; the carve-out this handle asked for
+    int last_l2_pf = 0;                               // L2 prefetch distance of the last launch (WN_PROF report)
     size_t wpack_bytes = 0;
     float* d_dense = nullptr;  size_t dense_bytes = 0;    // unfolded fp32 matrices of the batch forward (DenseLayout)
     float* d_fwd = nullptr;    size_t fwd_bytes = 0;      // wn_forward activation scratch
@@ -499,6 +501,31 @@ struct StreamCtx {
     const float* gbias;    // Wg . g, computed at open (NULL without global conditioning)
 };
 
+// How many streamed blobs the weight warp keeps in flight into L2 ahead of its shared-memory ring (wn_kernel.cuh
+// tma_loop).  The ring already puts each copy about nring stages ahead of its use; one more blob of lead through L2
+// is what measured best on an H100 (DESIGN.md 7: config 2 is 89.0 us/sample at D = 1, 89.6 at 2, 90.7 at 3, 92.6
+// at 6 and 102.9 at 8 against 94.4 at 0): prefetched blobs that wait longer in L2 evict each other, the exchange
+// and the conditioning weights.  D is capped by the grid-wide blob stages (P blocks x one blob) that fit in the L2
+// left once the persisting carve-out (the exchange buffer), history rings kept in global memory, the conditioning
+// weights (re-read every step) and a 2 MB margin are taken out; a handle counts on the share of that L2 its grid has
+// of the SMs, so the two half-grid handles of generate_concurrent, which run at the same time, split it.
+// WN_L2_PREFETCH=<D> overrides it (0: no prefetch).
+static int l2_prefetch_distance(const WnHandle* h, const WnPlan& pl) {
+    const int nstream = pl.nblobs - pl.nres;
+    if (nstream <= 0) return 0;
+    const int forced = env_int("WN_L2_PREFETCH", -1);
+    if (forced >= 0) return std::min(forced, nstream);
+    long long blob = 0;
+    for (int i = pl.nres; i < pl.nblobs; ++i) blob = std::max<long long>(blob, wn_blob_floats(pl, i) * 4LL);
+    const long long rings = pl.ring_in_smem ? 0 : (long long)pl.P * pl.ring_pos_total * pl.RA4 * pl.BT * 4;
+    long long budget = (long long)h->l2_bytes - (long long)h->l2_carve_bytes - rings - (long long)pl.P * pl.cta_cw_floats * 4 -
+                       (2LL << 20);
+    budget = budget * pl.P / std::max(h->num_sms, pl.P);
+    if (budget <= 0) return 0;
+    const int lead = 1;
+    return (int)std::min<long long>(std::min<long long>(budget / (pl.P * blob), lead), nstream);
+}
+
 static int32_t launch_chunk(WnHandle* h, const wn_generate_args* a, int b0, int Bc, cudaStream_t st,
                             const StreamCtx* sc = nullptr) {
     WnPlan pl;
@@ -507,6 +534,7 @@ static int32_t launch_chunk(WnHandle* h, const wn_generate_args* a, int b0, int 
     if (rc) return rc;
     if (pl.P != h->base.P || pl.lb_floats != h->base.lb_floats)
         return fail(WN_ERR_STATE, "plan changed between weight upload and generate");
+    pl.l2_pf = h->last_l2_pf = l2_prefetch_distance(h, pl);
     const int BT = pl.BT;
     const wn_config& c = h->cfg;
 
@@ -1091,6 +1119,7 @@ int32_t wn_create(const wn_config* cfg, void** handle) {
     h->engine = engine_choice();
     h->num_sms = prop.multiProcessorCount;
     h->smem_cap = (long long)prop.sharedMemPerBlockOptin;
+    h->l2_bytes = (size_t)prop.l2CacheSize;
     int32_t rc;
     if (h->engine == 7) {
         rc = build_plan7(h->cfg, 1, h->num_sms, h->smem_cap, h->base7, h->passes7, h->ringtab);
@@ -1111,6 +1140,7 @@ int32_t wn_create(const wn_config* cfg, void** handle) {
         const size_t want = h->l2_mode == 2 ? std::min<size_t>((size_t)prop.persistingL2CacheMaxSize, 16u << 20)
                                              : (size_t)prop.persistingL2CacheMaxSize;
         if (cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, want) == cudaSuccess) {
+            h->l2_carve_bytes = want;
             h->l2_persist_bytes = (size_t)prop.persistingL2CacheMaxSize;
             h->l2_window_max = (size_t)prop.accessPolicyMaxWindowSize;
         } else {
@@ -1322,6 +1352,7 @@ int32_t wn_sync(void* handle) {
             for (int p = 0; p < P; ++p) { mn = std::min(mn, pc[p * 16 + i]); mx = std::max(mx, pc[p * 16 + i]); sum += pc[p * 16 + i]; }
             fprintf(stderr, "WN_PROF %-20s mean %12.0f  min %12lld  max %12lld cycles\n", names[i], (double)sum / P, mn, mx);
         }
+        if (h->engine != 7) fprintf(stderr, "WN_PROF L2 prefetch distance %d blobs\n", h->last_l2_pf);
     }
     if (err[0] != 0) {
         cudaMemset(h->d_err, 0, sizeof(err));

@@ -141,6 +141,23 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
         "l"(src), "r"(bytes), "r"(smem_u32(bar))
         : "memory");
 }
+// the same copy with an L2 cache policy (createpolicy) attached to its reads
+__device__ __forceinline__ void bulk_g2s_hint(void* dst, const void* src, uint32_t bytes, uint64_t* bar, uint64_t pol) {
+    asm volatile(
+        "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(
+            smem_u32(dst)),
+        "l"(src), "r"(bytes), "r"(smem_u32(bar)), "l"(pol)
+        : "memory");
+}
+__device__ __forceinline__ uint64_t l2_policy_evict_first() {
+    uint64_t pol;
+    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+    return pol;
+}
+// ask L2 to fetch [src, src+bytes) from global memory (bytes a multiple of 16); no shared memory, no completion
+__device__ __forceinline__ void prefetch_l2(const void* src, uint32_t bytes) {
+    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src), "r"(bytes) : "memory");
+}
 __device__ __forceinline__ uint2 ld_pair(const uint2* p) {
     uint2 v;
     asm volatile("ld.relaxed.gpu.global.v2.u32 {%0,%1}, [%2];" : "=r"(v.x), "=r"(v.y) : "l"(p) : "memory");
@@ -665,7 +682,11 @@ struct Engine {
     }
 
     // ======================================================================================
-    // weight streaming warp
+    // weight streaming warp.  The streamed blobs (nres..L, every step) go through the shared-memory ring;
+    // the ring can only be pl.nring blobs deep, so in addition the warp asks L2 to fetch the blob pl.l2_pf
+    // places further along the same sequence (wrapping into the next step, never past the last step of the
+    // launch) before it issues each copy.  The ring copies read with an evict-first policy: a blob already
+    // in shared memory leaves L2 before the prefetched blobs that are still to be copied.
     // ======================================================================================
     __device__ void tma_loop() {
         if (lane != 0) return;
@@ -678,16 +699,27 @@ struct Engine {
         const int nstream = pl.nblobs - pl.nres;
         if (nstream <= 0) return;
         const uint32_t total = (uint32_t)pp.T * (uint32_t)nstream;
+        const uint32_t dist = (uint32_t)pl.l2_pf < total ? (uint32_t)pl.l2_pf : total;
+        int ipf = pl.nres;          // next blob to prefetch: dist blobs ahead of i
+        for (uint32_t k = 0; k < dist; ++k) {
+            prefetch_l2(base + wn_blob_off(pl, ipf), (uint32_t)wn_blob_floats(pl, ipf) * 4u);
+            if (++ipf == pl.nblobs) ipf = pl.nres;
+        }
+        const uint64_t pol = l2_policy_evict_first();
         int i = pl.nres;
         for (uint32_t js = 0; js < total; ++js) {
             const uint32_t s = js % (uint32_t)pl.nring, u = js / (uint32_t)pl.nring;
             if (u > 0) {
                 if (!wait_bar<true>(&bar_empty[s], (u - 1) & 1u, 0x40000000u | s)) return;
             }
+            if (dist > 0 && js + dist < total) {
+                prefetch_l2(base + wn_blob_off(pl, ipf), (uint32_t)wn_blob_floats(pl, ipf) * 4u);
+                if (++ipf == pl.nblobs) ipf = pl.nres;
+            }
             const uint32_t bytes = (uint32_t)wn_blob_floats(pl, i) * 4u;
             uint64_t* fb = &bar_full[pl.nres + s];
             mbar_expect_tx(fb, bytes);
-            bulk_g2s(slots + (size_t)(pl.nres + s) * pl.slot_floats, base + wn_blob_off(pl, i), bytes, fb);
+            bulk_g2s_hint(slots + (size_t)(pl.nres + s) * pl.slot_floats, base + wn_blob_off(pl, i), bytes, fb, pol);
             if (++i == pl.nblobs) i = pl.nres;
         }
     }

@@ -61,6 +61,7 @@ struct WnPlan {
     int nblobs;                 // L + 1 per step
     int nres;                   // blobs [0,nres) stay resident in shared memory for the whole call
     int nring;                  // the others stream through nring slots every step
+    int l2_pf;                  // streamed blobs the weight warp prefetches into L2 ahead of its ring copies (0: none)
     // ---- conditioning weights (kept in L2, read by the conditioning warp): [L][NQ_A][C][4]
     long long cta_cw_floats;
     // ---- exchange: element offsets (multiply by BT for pairs) of each vector inside one copy.
