@@ -1203,51 +1203,4 @@ wn7_kernel(const __grid_constant__ Wn7Plan pl, const __grid_constant__ Wn7Ptrs p
     else if (pl.C > 0) eng.cond_loop();
 }
 
-// gbias[b][l][row] = Wg_l[row,:] . g_b   (modules.py:148-152), once per call
-__global__ void wn7_gbias_kernel(const float* __restrict__ wg, const float* __restrict__ g, float* __restrict__ out,
-                                 int L, int G, int gin) {
-    const int l = blockIdx.x, b = blockIdx.y;
-    for (int row = threadIdx.x; row < G; row += blockDim.x) {
-        const float* w = wg + ((size_t)l * G + row) * gin;
-        float a = 0.f;
-        for (int i = 0; i < gin; ++i) a = fmaf(w[i], g[(size_t)b * gin + i], a);
-        out[((size_t)b * L + l) * G + row] = a;
-    }
-}
-
-// stand-alone samplers over (B,O,T): the reference's mixture.py entry points
-__global__ void wn7_sample_kernel(const float* __restrict__ y, int B, int O, int T, const float* __restrict__ u1,
-                                  const float* __restrict__ n2, float* __restrict__ out, int gauss) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= B * T) return;
-    const int b = i / T, t = i % T;
-    const float* yb = y + (size_t)b * O * T + t;
-    float mean, ls;
-    const int K = (O == 2) ? 1 : O / 3;
-    if (K > 1 || (!gauss)) {
-        float best = -INFINITY;
-        int bi = 0;
-        for (int k = 0; k < K; ++k) {
-            const float gk = yb[(size_t)k * T] - logf(-logf(u1[((size_t)t * B + b) * K + k]));
-            if (gk > best) {
-                best = gk;
-                bi = k;
-            }
-        }
-        mean = yb[(size_t)(K + bi) * T];
-        ls = yb[(size_t)(2 * K + bi) * T];
-    } else if (O == 2) {
-        mean = yb[0];
-        ls = yb[(size_t)T];
-    } else {
-        mean = yb[(size_t)T];
-        ls = yb[(size_t)2 * T];
-    }
-    const float v = n2[(size_t)t * B + b];
-    float xv;
-    if (!gauss) xv = __fadd_rn(mean, __fmul_rn(expf(ls), __fsub_rn(logf(v), logf(__fsub_rn(1.0f, v)))));
-    else xv = __fadd_rn(__fmul_rn(v, expf(ls)), mean);
-    out[i] = fminf(fmaxf(xv, -1.0f), 1.0f);
-}
-
 }  // namespace wn7

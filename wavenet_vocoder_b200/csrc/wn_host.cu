@@ -248,6 +248,18 @@ static int32_t build_plan(const wn_config& c, int batch, int num_sms, long long 
     return WN_OK;
 }
 
+// the work of one step, which depends on the model shape only: both kernel organisations report the same numbers
+static void fill_work(const wn_config& c, wn_plan_info* out) {
+    const int64_t R = c.residual_channels, G = c.gate_channels, G2 = G / 2, S = c.skip_channels, O = c.out_channels;
+    const int64_t L = c.layers, kw = c.kernel_size, C = c.cin_channels;
+    const int64_t cin0 = (c.input_kind == WN_INPUT_SCALAR) ? 1 : O;
+    // SURVEY.md 8(d): MAC = C0*R + L*(G*kw*R + G*C + S*G/2 + R*G/2) + S*S + O*S ; weights = MAC + biases
+    const int64_t mac = cin0 * R + L * (G * kw * R + G * C + S * G2 + R * G2) + S * S + O * S;
+    const int64_t biases = R + L * (G + S + R) + S + O;
+    out->flops_per_sample = 2 * mac;
+    out->weight_bytes_per_step = 4 * (mac + biases);
+}
+
 static void fill_info(const wn_config& c, const WnPlan& pl, wn_plan_info* out) {
     memset(out, 0, sizeof(*out));
     out->num_ctas = pl.P;
@@ -269,14 +281,7 @@ static void fill_info(const wn_config& c, const WnPlan& pl, wn_plan_info* out) {
     out->head_blob_bytes = (int64_t)pl.tb_floats * 4;
     out->packed_bytes_per_cta = (int64_t)pl.cta_w_floats * 4;
     out->cond_packed_bytes_per_cta = (int64_t)pl.cta_cw_floats * 4;
-    const int64_t cin0 = (c.input_kind == WN_INPUT_SCALAR) ? 1 : pl.O;
-    // SURVEY.md 8(d): MAC = C0*R + L*(G*kw*R + G*C + S*G/2 + R*G/2) + S*S + O*S ; weights = MAC + biases
-    const int64_t mac = cin0 * pl.R + (int64_t)pl.L * ((int64_t)pl.G * pl.kw * pl.R + (int64_t)pl.G * pl.C +
-                                                        (int64_t)pl.S * pl.G2 + (int64_t)pl.R * pl.G2) +
-                        (int64_t)pl.S * pl.S + (int64_t)pl.O * pl.S;
-    const int64_t biases = pl.R + (int64_t)pl.L * (pl.G + pl.S + pl.R) + pl.S + pl.O;
-    out->flops_per_sample = 2 * mac;
-    out->weight_bytes_per_step = 4 * (mac + biases);
+    fill_work(c, out);
     int64_t streamed = 0;
     for (int i = pl.nres; i < pl.nblobs; ++i) streamed += wn_blob_floats(pl, i) * 4LL;
     out->streamed_bytes_per_step = streamed * pl.P;
@@ -430,7 +435,8 @@ static int32_t check_weights(const wn_config& c, const wn_weights* w) {
 // which kernel organisation: 5 (default) = critical / deferred warp groups, values polled straight into the registers
 // of the threads that use them, quad-major GEMV + butterfly + one group barrier (csrc/wn_kernel.cuh); 7 = the
 // alternative: row-pair passes finalised inside the warp, up to 8 utterances per launch (csrc/wn7_kernel.cuh).
-// Both are parity-tested; measured on an H100 SXM (700 W): 95 us vs 111 us per sample for config 2 (DESIGN.md 7).
+// Both are parity-tested.  On an H100 SXM (700 W) 7 is 20 % slower at B = 1 (config 2) and 46 % faster for 8
+// utterances (config 4), which it runs in one launch (DESIGN.md 7).
 static int engine_choice() { return env_int("WN_ENGINE", 5) == 7 ? 7 : 5; }
 
 // ------------------------------------------------------------------------------------------
@@ -526,6 +532,39 @@ static int l2_prefetch_distance(const WnHandle* h, const WnPlan& pl) {
     return (int)std::min<long long>(std::min<long long>(budget / (pl.P * blob), lead), nstream);
 }
 
+// The per-call pointers and scalars of a launch of utterances [b0, b0 + Bc) of the call `a`; WnPtrs and Wn7Ptrs name
+// them alike.  C: conditioning channels, O: head outputs, K: mixture components.
+template <typename Ptrs>
+static void set_call_args(Ptrs& pp, const wn_generate_args* a, int b0, int Bc, int C, int O, int K) {
+    const int T = a->T, Tt = a->T_test;
+    pp.c = a->c ? a->c + (size_t)b0 * T * C : nullptr;
+    pp.initial = a->initial ? a->initial + b0 : nullptr;
+    pp.initial_dense = a->initial_dense ? a->initial_dense + (size_t)b0 * O : nullptr;
+    pp.initial_rows = a->initial_rows ? a->initial_rows + b0 : nullptr;
+    pp.test_scalar = a->test_scalar ? a->test_scalar + (size_t)b0 * Tt : nullptr;
+    pp.test_index = a->test_index ? a->test_index + (size_t)b0 * Tt : nullptr;
+    pp.test_dense = a->test_dense ? a->test_dense + (size_t)b0 * Tt * O : nullptr;
+    // noise is (T, Btotal, .): the kernel indexes with the total batch, so shift by the row
+    pp.u1 = a->noise_u1 ? a->noise_u1 + (size_t)b0 * K : nullptr;
+    pp.u2 = a->noise_u2 ? a->noise_u2 + b0 : nullptr;
+    pp.z = a->noise_z ? a->noise_z + b0 : nullptr;
+    pp.e = a->noise_e ? a->noise_e + (size_t)b0 * O : nullptr;
+    pp.out_scalar = a->out_scalar ? a->out_scalar + (size_t)b0 * T : nullptr;
+    pp.out_index = a->out_index ? a->out_index + (size_t)b0 * T : nullptr;
+    pp.out_dense = a->out_dense ? a->out_dense + (size_t)b0 * O * T : nullptr;
+    pp.params_out = a->params_out ? a->params_out + (size_t)b0 * O * T : nullptr;
+    pp.B = Bc;
+    pp.Btot = a->B;
+    pp.b0 = b0 + a->philox_row0;          // only the Philox counters use it (wn_kernel.cuh fetch_noise)
+    pp.T = T;
+    pp.T_test = Tt;
+    pp.initial_index = a->initial_index < 0 ? 127 : a->initial_index;   // wavenet.py:286
+    pp.flags = a->flags;
+    pp.noise_kind = a->noise_kind;
+    pp.seed = a->seed;
+    pp.timeout_cycles = (long long)env_int("WN_TIMEOUT_MS", 2000) * 1500000LL;
+}
+
 static int32_t launch_chunk(WnHandle* h, const wn_generate_args* a, int b0, int Bc, cudaStream_t st,
                             const StreamCtx* sc = nullptr) {
     WnPlan pl;
@@ -567,7 +606,6 @@ static int32_t launch_chunk(WnHandle* h, const wn_generate_args* a, int b0, int 
         h->launches++;
         pp.gbias = h->d_gbias;
     }
-    const int T = a->T, Tt = a->T_test, O = pl.O, K = pl.Kmix;
     pp.wpack = h->d_wpack;
     pp.cwpack = h->d_cwpack;
     pp.first_w = h->d_first_w;
@@ -576,32 +614,7 @@ static int32_t launch_chunk(WnHandle* h, const wn_generate_args* a, int b0, int 
     pp.ring_g = (sc && !pl.ring_in_smem) ? sc->state : h->d_ring;
     pp.ringtab = h->d_ringtab;
     pp.err = h->d_err;
-    pp.c = a->c ? a->c + (size_t)b0 * T * pl.C : nullptr;
-    pp.initial = a->initial ? a->initial + b0 : nullptr;
-    pp.initial_dense = a->initial_dense ? a->initial_dense + (size_t)b0 * O : nullptr;
-    pp.initial_rows = a->initial_rows ? a->initial_rows + b0 : nullptr;
-    pp.test_scalar = a->test_scalar ? a->test_scalar + (size_t)b0 * Tt : nullptr;
-    pp.test_index = a->test_index ? a->test_index + (size_t)b0 * Tt : nullptr;
-    pp.test_dense = a->test_dense ? a->test_dense + (size_t)b0 * Tt * O : nullptr;
-    // noise is (T, Btotal, .): the kernel indexes with the total batch, so shift by the row
-    pp.u1 = a->noise_u1 ? a->noise_u1 + (size_t)b0 * K : nullptr;
-    pp.u2 = a->noise_u2 ? a->noise_u2 + b0 : nullptr;
-    pp.z = a->noise_z ? a->noise_z + b0 : nullptr;
-    pp.e = a->noise_e ? a->noise_e + (size_t)b0 * O : nullptr;
-    pp.out_scalar = a->out_scalar ? a->out_scalar + (size_t)b0 * T : nullptr;
-    pp.out_index = a->out_index ? a->out_index + (size_t)b0 * T : nullptr;
-    pp.out_dense = a->out_dense ? a->out_dense + (size_t)b0 * O * T : nullptr;
-    pp.params_out = a->params_out ? a->params_out + (size_t)b0 * O * T : nullptr;
-    pp.B = Bc;
-    pp.Btot = a->B;
-    pp.b0 = b0 + a->philox_row0;          // only the Philox counters use it (wn_kernel.cuh fetch_noise)
-    pp.T = T;
-    pp.T_test = Tt;
-    pp.initial_index = a->initial_index < 0 ? 127 : a->initial_index;   // wavenet.py:286
-    pp.flags = a->flags;
-    pp.noise_kind = a->noise_kind;
-    pp.seed = a->seed;
-    pp.timeout_cycles = (long long)env_int("WN_TIMEOUT_MS", 2000) * 1500000LL;
+    set_call_args(pp, a, b0, Bc, pl.C, pl.O, pl.Kmix);
     pp.warp_reverse = env_int("WN_WARP_REVERSE", 0);
     pp.gate_cycles = env_int("WN_GATE_CYCLES", 0);
     pp.fast_gate = env_int("WN_FAST_GATE", 0);
@@ -724,14 +737,7 @@ static void fill_info7(const wn_config& c, const Wn7Plan& pl, wn_plan_info* out)
     out->poll_warps = pl.npw;
     out->num_passes = pl.npass;
     out->engine = 7;
-    const int64_t cin0 = (c.input_kind == WN_INPUT_SCALAR) ? 1 : pl.O;
-    // SURVEY.md 8(d): MAC = C0*R + L*(G*kw*R + G*C + S*G/2 + R*G/2) + S*S + O*S ; weights = MAC + biases
-    const int64_t mac = cin0 * pl.R + (int64_t)pl.L * ((int64_t)pl.G * pl.kw * pl.R + (int64_t)pl.G * pl.C +
-                                                        (int64_t)pl.S * pl.G2 + (int64_t)pl.R * pl.G2) +
-                        (int64_t)pl.S * pl.S + (int64_t)pl.O * pl.S;
-    const int64_t biases = pl.R + (int64_t)pl.L * (pl.G + pl.S + pl.R) + pl.S + pl.O;
-    out->flops_per_sample = 2 * mac;
-    out->weight_bytes_per_step = 4 * (mac + biases);
+    fill_work(c, out);
     int64_t streamed = 0;
     for (int i = pl.nres; i < pl.nblobs; ++i) streamed += wn7_blob_floats(pl, i) * 4LL;
     out->streamed_bytes_per_step = streamed * pl.P;
@@ -821,13 +827,12 @@ static int32_t launch_chunk7(WnHandle* h, const wn_generate_args* a, int b0, int
         const size_t gb = (size_t)Bc * pl.L * pl.G * sizeof(float);
         rc = ensure(&h->d_gbias, &h->gbias_bytes, gb);
         if (rc) return rc;
-        wn7::wn7_gbias_kernel<<<dim3(pl.L, Bc), 128, 0, st>>>(h->d_wg, a->g + (size_t)b0 * c.gin_channels, h->d_gbias,
-                                                            pl.L, pl.G, c.gin_channels);
+        wn::wn_gbias_kernel<<<dim3(pl.L, Bc), 128, 0, st>>>(h->d_wg, a->g + (size_t)b0 * c.gin_channels, h->d_gbias,
+                                                          pl.L, pl.G, c.gin_channels);
         CUDA_TRY(cudaGetLastError());
         h->launches++;
         pp.gbias = h->d_gbias;
     }
-    const int T = a->T, Tt = a->T_test, O = pl.O, K = pl.Kmix;
     pp.wpack = h->d_wpack;
     pp.cwpack = h->d_cwpack;
     pp.bpack = h->d_bpack;
@@ -840,32 +845,7 @@ static int32_t launch_chunk7(WnHandle* h, const wn_generate_args* a, int b0, int
     pp.ring_g = h->d_ring;
     pp.ringtab = h->d_ringtab;
     pp.err = h->d_err;
-    pp.c = a->c ? a->c + (size_t)b0 * T * pl.C : nullptr;
-    pp.initial = a->initial ? a->initial + b0 : nullptr;
-    pp.initial_dense = a->initial_dense ? a->initial_dense + (size_t)b0 * O : nullptr;
-    pp.initial_rows = a->initial_rows ? a->initial_rows + b0 : nullptr;
-    pp.test_scalar = a->test_scalar ? a->test_scalar + (size_t)b0 * Tt : nullptr;
-    pp.test_index = a->test_index ? a->test_index + (size_t)b0 * Tt : nullptr;
-    pp.test_dense = a->test_dense ? a->test_dense + (size_t)b0 * Tt * O : nullptr;
-    // noise is (T, Btotal, .): the kernel indexes with the total batch, so shift by the row
-    pp.u1 = a->noise_u1 ? a->noise_u1 + (size_t)b0 * K : nullptr;
-    pp.u2 = a->noise_u2 ? a->noise_u2 + b0 : nullptr;
-    pp.z = a->noise_z ? a->noise_z + b0 : nullptr;
-    pp.e = a->noise_e ? a->noise_e + (size_t)b0 * O : nullptr;
-    pp.out_scalar = a->out_scalar ? a->out_scalar + (size_t)b0 * T : nullptr;
-    pp.out_index = a->out_index ? a->out_index + (size_t)b0 * T : nullptr;
-    pp.out_dense = a->out_dense ? a->out_dense + (size_t)b0 * O * T : nullptr;
-    pp.params_out = a->params_out ? a->params_out + (size_t)b0 * O * T : nullptr;
-    pp.B = Bc;
-    pp.Btot = a->B;
-    pp.b0 = b0 + a->philox_row0;
-    pp.T = T;
-    pp.T_test = Tt;
-    pp.initial_index = a->initial_index < 0 ? 127 : a->initial_index;   // wavenet.py:286
-    pp.flags = a->flags;
-    pp.noise_kind = a->noise_kind;
-    pp.seed = a->seed;
-    pp.timeout_cycles = (long long)env_int("WN_TIMEOUT_MS", 2000) * 1500000LL;
+    set_call_args(pp, a, b0, Bc, pl.C, pl.O, pl.Kmix);
     pp.prof = nullptr;
     if (env_int("WN_PROF", 0)) {
         const size_t pb = (size_t)pl.P * 16 * sizeof(long long);
