@@ -71,7 +71,8 @@ typedef struct wn_config {
     int32_t num_ctas;             /* 0 = choose; else number of cooperating thread blocks */
     int32_t exchange_copies;      /* 0 = choose; replicas of each exchange vector in L2   */
     int32_t ring_slots;           /* 0 = choose; streaming weight slots in shared memory  */
-    int32_t poll_warps;           /* 0 = choose; warps that poll the exchange into shared memory (2..12) */
+    int32_t poll_warps;           /* 0 = choose; warps that poll the exchange into shared memory (2..8, larger
+                                     values plan as 8); -1 = none, the compute warps poll (engine 7) */
     int32_t reserved[7];
 } wn_config;
 

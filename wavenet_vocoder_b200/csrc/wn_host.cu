@@ -281,6 +281,7 @@ static void fill_info(const wn_config& c, const WnPlan& pl, wn_plan_info* out) {
     out->head_blob_bytes = (int64_t)pl.tb_floats * 4;
     out->packed_bytes_per_cta = (int64_t)pl.cta_w_floats * 4;
     out->cond_packed_bytes_per_cta = (int64_t)pl.cta_cw_floats * 4;
+    out->engine = 5;
     fill_work(c, out);
     int64_t streamed = 0;
     for (int i = pl.nres; i < pl.nblobs; ++i) streamed += wn_blob_floats(pl, i) * 4LL;
@@ -1364,7 +1365,6 @@ int32_t wn_get_plan(void* handle, int32_t batch, wn_plan_info* out) {
     if (rc) return rc;
     fill_info(h->cfg, pl, out);
     out->launches = h->launches;
-    out->engine = 5;
     return WN_OK;
 }
 

@@ -1078,9 +1078,11 @@ struct Engine {
         // ---- lean stage path (pl.lean, set by wn_host.cu: one utterance, exact vector lengths, one gate quad and one
         // residual quad per block).  A stage is a chain of dependent instructions executed by one warp per SM
         // sub-partition, each waiting for the one before, so what a stage costs beyond the
-        // exchange is its LENGTH IN INSTRUCTIONS: same arithmetic and order as the generic loop below, with every
-        // address that does not depend on the stage computed once here, no per-element bounds checks, and the spin
-        // loops out of line.
+        // exchange is its LENGTH IN INSTRUCTIONS: same arithmetic as the generic loop below, with every address that
+        // does not depend on the stage computed once here, no per-element bounds checks, and the spin loops out of
+        // line.  One difference in order: a stage adds its x product (V x, formed while y is still travelling) to
+        // the accumulator before its y product (M y); the generic loop adds it after.  So the two paths agree to
+        // fp32 rounding, not bit for bit (tests/test_plan_variants.py).
         constexpr bool LEAN_T = LEAN;
         constexpr bool lean = LEAN;
         constexpr int LY = LEAN_T ? EG / 2 : 1, LX = LEAN_T ? ER / 2 : 1;

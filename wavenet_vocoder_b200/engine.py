@@ -74,8 +74,9 @@ def weights_struct(sd: Dict[str, torch.Tensor], layers: int, cin: int, gin: int)
 
 def make_config(*, layers, stacks, residual_channels, gate_channels, skip_out_channels, out_channels,
                 kernel_size, cin_channels, gin_channels, scalar_input, output_distribution,
-                device_index=0, num_ctas=0):
-    """wn_config from the reference's constructor keywords (wavenet.py:98-111)."""
+                device_index=0, num_ctas=0, exchange_copies=0, ring_slots=0, poll_warps=0):
+    """wn_config from the reference's constructor keywords (wavenet.py:98-111).  num_ctas, exchange_copies,
+    ring_slots and poll_warps are the planner's fields of include/wn.h (0 = the planner chooses)."""
     if scalar_input:
         if output_distribution == "Logistic":
             head = N.WN_HEAD_MOL
@@ -96,6 +97,7 @@ def make_config(*, layers, stacks, residual_channels, gate_channels, skip_out_ch
     cfg.head_kind = head
     cfg.device = int(device_index)
     cfg.num_ctas = int(num_ctas)
+    cfg.exchange_copies, cfg.ring_slots, cfg.poll_warps = int(exchange_copies), int(ring_slots), int(poll_warps)
     return cfg
 
 
@@ -305,7 +307,8 @@ class SynthesisEngine:
 
     def __init__(self, *, layers, stacks, residual_channels, gate_channels, skip_out_channels,
                  out_channels, kernel_size, cin_channels, gin_channels, scalar_input,
-                 output_distribution, device: torch.device, num_ctas=0):
+                 output_distribution, device: torch.device, num_ctas=0, exchange_copies=0, ring_slots=0,
+                 poll_warps=0):
         if device.type != "cuda":
             raise RuntimeError("wavenet_vocoder_b200 runs the synthesis path on a CUDA device only "
                                "(there is no CPU fallback); got device %s" % device)
@@ -320,7 +323,8 @@ class SynthesisEngine:
                           gin_channels=gin_channels, scalar_input=scalar_input,
                           output_distribution=output_distribution,
                           device_index=device.index if device.index is not None else torch.cuda.current_device(),
-                          num_ctas=num_ctas)
+                          num_ctas=num_ctas, exchange_copies=exchange_copies, ring_slots=ring_slots,
+                          poll_warps=poll_warps)
         self.head = head = cfg.head_kind
         self.K = 0 if head == N.WN_HEAD_SOFTMAX else (1 if out_channels == 2 else out_channels // 3)
         self.cfg = cfg
@@ -330,7 +334,8 @@ class SynthesisEngine:
         self._ctor = dict(layers=layers, stacks=stacks, residual_channels=residual_channels, gate_channels=gate_channels,
                           skip_out_channels=skip_out_channels, out_channels=out_channels, kernel_size=kernel_size,
                           cin_channels=cin_channels, gin_channels=gin_channels, scalar_input=scalar_input,
-                          output_distribution=output_distribution, device=device)
+                          output_distribution=output_distribution, device=device,
+                          exchange_copies=exchange_copies, ring_slots=ring_slots, poll_warps=poll_warps)
         self._sd = None
         self._halves = None           # two half-grid engines for concurrent batch tiles (see generate_concurrent)
         self._is_child = num_ctas > 0
