@@ -1,10 +1,10 @@
 # coding: utf-8
 """The plan-variant matrix: model shapes x batch x knob settings that move the synthesis kernel's pipeline without
 changing the model -- the weight ring's depth and resident / streamed split, the L2 prefetch distance, history rings in
-global memory, exchange replicas and layout, warp order and poll timing, engine 7's polling warps, the batch tile and
-the lean stage path.  Shared by tests/test_plan_variants_host.py (every entry's plan and the kernel instantiation it
-launches, without a GPU) and tests/test_plan_variants.py (every entry on an H100, against the default plan of the same
-shape and against float64 forward()).
+global memory, exchange replicas and layout, warp order and poll timing, engine 7's polling warps and the batch
+tile.  Shared by tests/test_plan_variants_host.py (every entry's plan and the kernel instantiation it launches, without
+a GPU) and tests/test_plan_variants.py (every entry on an H100, against the default plan of the same shape and against
+float64 forward()).
 
 Every knob is read when a handle is planned, so each entry runs on a handle of its own created under its settings.
 An entry is checked bit for bit against the default plan (``bit`` is None) wherever the knob only moves data or
@@ -44,9 +44,6 @@ STREAM_SPLIT = (1, 7, 64)
 SHORT_T = (1, 2)
 
 NUM_CTAS_WHY = "the row partition changes, and with it every GEMV's summation order"
-FAST_GATE_WHY = "the gate's ex2.approx / rcp.approx differ from expf / division by about 1e-6"
-LEAN_WHY = ("the lean stage path adds a stage's x product (V x) to the accumulator before its y product (M y), the "
-            "generic path after it (wn_kernel.cuh crit_loop): the last bits differ")
 TILE1_WHY = ("at a tile of 1 a thread owns pairs of adjacent vector elements, at 2, 4 and 8 every 128th one "
              "(wn_kernel.cuh elem): where a thread holds two or more elements its partial sums differ in the last bits")
 
@@ -57,13 +54,12 @@ class Entry:
     at T = 1 and 2 (against the first steps of its own long run); stream: also run as a stream in chunks (engine 5,
     B <= 4), against its own one-shot run; vs_b1: row 0 also equals the default plan at B = 1 bit for bit (every
     element of a row is summed in the same order whatever the tile: the tile is 1, or a thread holds one element
-    of each vector); ref_env: the knobs of the plan the entry is compared with (default: none)."""
+    of each vector)."""
 
     def __init__(self, id, base, B=1, engine=5, env=None, cfg=None, expect=None, bit=None, short=False, stream=False,
-                 vs_b1=False, ref_env=None):
+                 vs_b1=False):
         self.id, self.base, self.B, self.engine = id, base, B, engine
         self.env = {k: str(v) for k, v in (env or {}).items()}
-        self.ref_env = {k: str(v) for k, v in (ref_env or {}).items()}
         self.cfg = dict(cfg or {})
         self.expect = dict(expect or {})
         self.bit, self.short, self.stream, self.vs_b1 = bit, short, stream, vs_b1
@@ -107,11 +103,6 @@ MATRIX = [
     _e("cfg2_ncopy16_cfg", "cfg2", cfg=dict(exchange_copies=16), expect=dict(exchange_copies=16)),
     _e("cfg2_warp_reverse", "cfg2", env={"WN_WARP_REVERSE": 1}, expect=_C2S),
     _e("cfg2_gate_cycles", "cfg2", env={"WN_GATE_CYCLES": 3000}, expect=_C2S),
-    # the lean stage path, and a poll delay on it (against the lean path without one)
-    _e("cfg2_lean", "cfg2", env={"WN_LEAN": 1}, expect=_C2S, bit=LEAN_WHY, short=True, stream=True),
-    _e("cfg2_lean_gate_cycles", "cfg2", env={"WN_LEAN": 1, "WN_GATE_CYCLES": 3000}, expect=_C2S,
-       ref_env={"WN_LEAN": 1}),
-    _e("cfg2_lean_fast_gate", "cfg2", env={"WN_LEAN": 1, "WN_FAST_GATE": 1}, expect=_C2S, bit=FAST_GATE_WHY),
     # block count: 64; 100 = 3 gate rows per block (a half-filled quad), no resident blob, 3 ring slots
     _e("cfg2_ctas64", "cfg2", env={"WN_NUM_CTAS": 64}, expect=dict(num_ctas=64), bit=NUM_CTAS_WHY),
     _e("cfg2_ctas100", "cfg2", env={"WN_NUM_CTAS": 100},
@@ -136,9 +127,6 @@ MATRIX = [
        stream=True),
 
     # ---------------- engine 5, config 5 (rings in global memory)
-    _e("cfg5_lean", "cfg5", env={"WN_LEAN": 1}, expect=dict(rings_in_smem=0), bit=LEAN_WHY, stream=True),
-    _e("cfg5_lean_fast_gate", "cfg5", env={"WN_LEAN": 1, "WN_FAST_GATE": 1}, expect=dict(rings_in_smem=0),
-       bit=FAST_GATE_WHY),
     _e("cfg5_ring2", "cfg5", env={"WN_RING_SLOTS": 2}, expect=dict(ring_slots=2, resident_blobs=6)),
     _e("cfg5_resident0", "cfg5", env={"WN_RESIDENT": 0}, expect=dict(ring_slots=4, resident_blobs=0)),
     _l2pf("cfg5", 2, dict(ring_slots=4, resident_blobs=4, rings_in_smem=0)),
@@ -225,7 +213,6 @@ def existing_launches():
         ("tests/test_streaming.py::test_golden_cases_chunked_equal_one_shot[mol_cond-3-replay]", mol, 3, 5, True, {}),
         ("tests/test_streaming.py::test_rings_in_global_memory[1]", c5, 1, 5, True, {}),
         ("tests/test_streaming.py::test_rings_in_global_memory[3]", c5, 3, 5, True, {}),
-        ("tests/test_streaming.py::test_lean_kernel", c2, 1, 5, True, {"WN_LEAN": "1"}),
     ]
     return out
 
@@ -251,30 +238,12 @@ def variant(R, G2):
     return 8, 8
 
 
-def lean_eligible(kw, plan, env):
-    """launch_chunk's condition for the lean stage path, from the model and its plan."""
-    R, G2, S, O, L = kw["residual_channels"], kw["gate_channels"] // 2, kw["skip_out_channels"], kw["out_channels"], \
-        kw["layers"]
-    er, eg = variant(R, G2)
-    chunk = 1 << int(env.get("WN_XC_SHIFT", 5))
-    xstride = int(env.get("WN_XSTRIDE", 544))
-    ex_sk = L * (G2 + R)
-    return (int(env.get("WN_LEAN", 0)) != 0 and plan["batch_tile"] == 1 and (er, eg) in ((2, 2), (4, 2)) and
-            plan["exchange_copies"] == 1 and kw["kernel_size"] == 3 and plan["rows_y"] == 2 and
-            plan["rows_x"] <= 4 and plan["rows_skip"] <= 4 and L >= 2 and er * 128 == R and eg * 128 == G2 and
-            (G2 + R) % chunk == 0 and G2 % chunk == 0 and xstride % 2 == 0 and S == G2 and
-            plan["rows_head_a"] <= 4 and plan["rows_head_b"] <= 4 and O <= 128 and ex_sk % chunk == 0 and
-            (ex_sk + S) % chunk == 0)
-
-
-def kernel_name(kw, plan, engine, stream, env):
+def kernel_name(kw, plan, engine, stream):
     """The kernel instantiation a launch with this plan takes, as `nm -C` spells its host stub."""
     if engine == 7:
         return "wn7::wn7_kernel<%d, %s>" % (plan["batch_tile"], "true" if plan["poll_warps"] == 0 else "false")
     er, eg = variant(kw["residual_channels"], kw["gate_channels"] // 2)
-    lean = lean_eligible(kw, plan, env)
-    return "wn::wn_persistent_kernel<%d, %d, %d, %s, %s>" % (plan["batch_tile"], er, eg, "true" if lean else "false",
-                                                            "true" if stream else "false")
+    return "wn::wn_persistent_kernel<%d, %d, %d, %s>" % (plan["batch_tile"], er, eg, "true" if stream else "false")
 
 
 def max_tile(env, engine):

@@ -763,29 +763,3 @@ def test_concurrent_half_grid_tiles_equal_sequential_tiles():
     y = mc.incremental_forward(c=c.transpose(1, 2).contiguous(), T=T, seed=99)
     assert tuple(y.shape) == (B, 1, T)
     assert float(((y[:, 0] - ref) ** 2).mean().sqrt()) <= RMS_TOL
-
-
-def test_lean_stage_path_against_oracle_and_generic(monkeypatch):
-    """The lean variant of the engine-5 kernel (WN_LEAN=1: hoisted addressing, residual rows published by the deferred
-    group; an experiment that is off by default, DESIGN.md section 7) on BASELINE config 2's shape: teacher-forced head
-    outputs against the oracle, and the free-running waveform against the default kernel."""
-    m, cfg, w, _ = full_case("cfg2_mol24")
-    T, B = 160, 1
-    gen = torch.Generator().manual_seed(2)
-    c = torch.randn(B, cfg.cin_channels, T, generator=gen)
-    noise = orc.predraw_noise(cfg, B, T, 4)
-    rec = []
-    with torch.no_grad():
-        y_ref = orc.incremental_forward(cfg, w, c=c, T=T, noise=orc.replay_from_predrawn(cfg, noise), params_out=rec)
-    p_ref = torch.stack(rec, dim=-1)
-    mc = m.cuda()
-    ti = torch.cat([torch.zeros(B, 1, 1), y_ref[:, :, :-1]], dim=2)
-    y_gen = mc.incremental_forward(c=c, T=T, noise=dev_noise(noise)).cpu()
-    monkeypatch.setenv("WN_LEAN", "1")
-    assert mc._get_engine().plan(1)["engine"] == 5
-    _, params = mc.incremental_forward(test_inputs=ti, c=c, T=T, noise=dev_noise(noise), return_params=True)
-    y_lean = mc.incremental_forward(c=c, T=T, noise=dev_noise(noise)).cpu()
-    monkeypatch.delenv("WN_LEAN")
-    assert float((params.cpu() - p_ref).abs().max()) <= PARAM_TOL * 2
-    assert float(((y_lean - y_ref) ** 2).mean().sqrt()) <= RMS_TOL
-    assert float(((y_lean - y_gen) ** 2).mean().sqrt()) <= RMS_TOL

@@ -8,9 +8,8 @@ the entry's knobs, checked two ways:
   (b) the teacher-forced head outputs against the module's float64 batch forward();
 and, where the entry asks for it, bit for bit against its own long run at T = 1 and 2 (its first steps) and as a
 stream cut into chunks of 1, 7 and 64 samples.  Entries whose knob changes the arithmetic or its order (the row
-partition, the approximate gate, the lean path's order of the two products, a tile of 1) are compared with the default
-plan through (b) alone; the entry says why.  A race, a wrong ring slot or a stale exchange line cannot hide inside
-(a)'s tolerance, because it has none."""
+partition, a tile of 1) are compared with the default plan through (b) alone; the entry says why.  A race, a wrong
+ring slot or a stale exchange line cannot hide inside (a)'s tolerance, because it has none."""
 import os
 
 import pytest
@@ -162,13 +161,11 @@ def assert_equal(got, ref, what):
 _DEFAULTS = {}
 
 
-def default_runs(d, B, engine, monkeypatch, env=None):
-    """The same shape, batch and inputs on a handle of the default plan, or of the plan under `env` (one per base,
-    batch, engine and env)."""
-    env = env or {}
-    key = (d.base, B, engine, tuple(sorted(env.items())))
+def default_runs(d, B, engine, monkeypatch):
+    """The same shape, batch and inputs on a handle of the default plan (one per base, batch and engine)."""
+    key = (d.base, B, engine)
     if key not in _DEFAULTS:
-        eng = new_engine(d, engine, env, {}, monkeypatch)
+        eng = new_engine(d, engine, {}, {}, monkeypatch)
         try:
             _DEFAULTS[key] = runs(eng, d, B)
         finally:
@@ -179,7 +176,7 @@ def default_runs(d, B, engine, monkeypatch, env=None):
 @pytest.mark.parametrize("e", pv.MATRIX, ids=[e.id for e in pv.MATRIX])
 def test_plan_variant(e, bases, monkeypatch):
     d = bases(e.base)
-    ref = default_runs(d, e.B, e.engine, monkeypatch, e.ref_env) if e.bit is None else None
+    ref = default_runs(d, e.B, e.engine, monkeypatch) if e.bit is None else None
     ref1 = default_runs(d, 1, e.engine, monkeypatch) if e.vs_b1 else None
     eng = new_engine(d, e.engine, e.env, e.cfg, monkeypatch)
     try:

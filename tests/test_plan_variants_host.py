@@ -63,7 +63,7 @@ def launches(kw, B, engine, stream, env, cfg=None):
     out = []
     for b in sorted(set(sizes)):
         p = plan_only(kw, b, **(cfg or {}))
-        out.append((p, pv.kernel_name(kw, p, engine, stream, env)))
+        out.append((p, pv.kernel_name(kw, p, engine, stream)))
     return out
 
 
@@ -93,8 +93,6 @@ def test_entry_plans_what_it_tests(e, monkeypatch):
         assert (p["ring_slots"] > 0) == (nstream > 0)
         if any(k in e.env for k in ("WN_L2_PREFETCH", "WN_RING_SLOTS", "WN_RESIDENT")) or "ring_slots" in e.cfg:
             assert nstream > 0, "%s: nothing is streamed, the knob has nothing to act on" % e.id
-        if "WN_LEAN" in e.env:
-            assert ", true, " in kernel, "%s: the lean stage path is not taken" % e.id
         if e.engine == 7 and ("poll_warps" in e.cfg or "WN_POLL_WARPS" in e.env):
             assert kernel.endswith("false>"), "%s: the polling-warp kernel is not taken" % e.id
         # the variant follows R and G/2 (wn_host.cu launch_chunk's efor)
@@ -139,7 +137,7 @@ def library_kernels():
     if nm is None:
         pytest.skip("nm (binutils) is not installed: the kernel instantiations cannot be listed")
     out = subprocess.run([nm, "-C", path], capture_output=True, text=True, check=True).stdout
-    return set(re.findall(r"(wn::wn_persistent_kernel<\d+, \d+, \d+, (?:true|false), (?:true|false)>|"
+    return set(re.findall(r"(wn::wn_persistent_kernel<\d+, \d+, \d+, (?:true|false)>|"
                           r"wn7::wn7_kernel<\d+, (?:true|false)>)", out))
 
 

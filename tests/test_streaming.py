@@ -1,8 +1,8 @@
 # coding: utf-8
 """Streaming synthesis on the GPU: an utterance made chunk by chunk (WaveNet.open_stream, wn_stream_* of the C ABI)
 is bit-identical to the same utterance made by one incremental_forward call, for irregular splits, replayed and
-Philox noise, batch tiles of 1, 3 and 4, both ring placements, the lean kernel, conditioning frames pushed in groups,
-and interleaved streams; StreamDecoder equals decode_device bit for bit; every misuse is refused."""
+Philox noise, batch tiles of 1, 3 and 4, both ring placements, conditioning frames pushed in groups, and interleaved
+streams; StreamDecoder equals decode_device bit for bit; every misuse is refused."""
 import ctypes as C
 
 import pytest
@@ -121,8 +121,6 @@ def test_golden_cases_chunked_equal_one_shot(name, B, noise_kind):
     assert_same(chunked(m, gc.kw, B, T, init, c, g, noise, seed), one_shot(m, B, T, init, c, g, noise, seed))
 
 
-CFG2 = dict(out_channels=30, layers=24, stacks=4, residual_channels=512, gate_channels=512, skip_out_channels=256,
-            cin_channels=80, gin_channels=-1, scalar_input=True, output_distribution="Logistic", dropout=0.0)
 CFG5 = dict(out_channels=30, layers=30, stacks=3, residual_channels=256, gate_channels=512, skip_out_channels=256,
             cin_channels=80, gin_channels=-1, scalar_input=True, output_distribution="Logistic", dropout=0.0)
 
@@ -145,18 +143,6 @@ def test_rings_in_global_memory(B):
     init, c, g = inputs_for(m, CFG5, B, T, gen)
     for noise, seed in ((cfg_noise(CFG5, B, T, 8), None), (None, 77)):
         assert_same(chunked(m, CFG5, B, T, init, c, g, noise, seed), one_shot(m, B, T, init, c, g, noise, seed))
-
-
-def test_lean_kernel(monkeypatch):
-    """WN_LEAN=1 on config 2's shape (the lean instantiation of the kernel)."""
-    monkeypatch.setenv("WN_LEAN", "1")
-    m = model_of(CFG2)
-    assert m._get_engine().plan(1)["rings_in_smem"] == 1
-    T = 2 * max_dilation(CFG2) + 150
-    gen = torch.Generator().manual_seed(4)
-    init, c, g = inputs_for(m, CFG2, 1, T, gen)
-    for noise, seed in ((cfg_noise(CFG2, 1, T, 9), None), (None, 55)):
-        assert_same(chunked(m, CFG2, 1, T, init, c, g, noise, seed), one_shot(m, 1, T, init, c, g, noise, seed))
 
 
 def upsample_model(scales, cin_pad, C=16):

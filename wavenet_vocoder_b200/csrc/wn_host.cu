@@ -208,7 +208,9 @@ static int32_t build_plan(const wn_config& c, int batch, int num_sms, long long 
         const int nq1 = std::max(pl.NQ_A + pl.NQ_BO, std::max(pl.NQ_BS, std::max(pl.NQ_HA, pl.NQ_HB)));
         pl.red1_floats = nq1 * 4 * BT * 4 + 4;                // partial sums of the 4 warps of a group
         pl.sm_red1 = take(2LL * pl.red1_floats * 4, 16);
-        pl.red2_floats = (pl.NQ_D + pl.NQ_BS + pl.NQ_BO) * 4 * BT * 4 + 4;   // + the residual rows (lean path, def_loop)
+        // + NQ_BO quads that no kernel writes: without them the fit below changes (config 5 at a batch tile of 8 would
+        // keep 3 blobs resident instead of 2), and the resident / streamed split is a tuning decision of its own
+        pl.red2_floats = (pl.NQ_D + pl.NQ_BS + pl.NQ_BO) * 4 * BT * 4 + 4;
         pl.sm_red2 = take(2LL * pl.red2_floats * 4, 16);      // two buffers each, alternating by stage
         pl.sm_sb = take(2LL * pl.L * pl.RA4 * BT * 4, 16);     // static part + per-step pre-sum table
         pl.sm_cond = take(pl.C > 0 ? 2LL * pl.L * pl.RA4 * BT * 4 : 16, 16);
@@ -476,7 +478,7 @@ struct WnHandle {
     cudaStream_t last_stream = nullptr;
     bool pending = false;
     int64_t launches = 0;
-    bool attr_set[40] = {};       // [20, 40): the stream instantiations
+    bool attr_set[28] = {};       // [0, 16): whole utterances, [16, 28): the stream instantiations
     size_t l2_persist_bytes = 0, l2_window_max = 0;   // persisting-L2 carve-out
     int l2_mode = 0;                                  // WN_L2_PERSIST: 1 = packed weights, 2 = exchange buffer
     size_t l2_bytes = 0, l2_carve_bytes = 0;          // L2 size; the carve-out this handle asked for
@@ -618,7 +620,6 @@ static int32_t launch_chunk(WnHandle* h, const wn_generate_args* a, int b0, int 
     set_call_args(pp, a, b0, Bc, pl.C, pl.O, pl.Kmix);
     pp.warp_reverse = env_int("WN_WARP_REVERSE", 0);
     pp.gate_cycles = env_int("WN_GATE_CYCLES", 0);
-    pp.fast_gate = env_int("WN_FAST_GATE", 0);
     pp.prof = nullptr;
     if (env_int("WN_PROF", 0)) {
         const size_t pb = (size_t)pl.P * 16 * sizeof(long long);
@@ -633,26 +634,13 @@ static int32_t launch_chunk(WnHandle* h, const wn_generate_args* a, int b0, int 
     auto efor = [](int K) { return K <= 128 ? 1 : (K <= 256 ? 2 : (K <= 512 ? 4 : 8)); };
     const int er = efor(pl.R), eg = efor(pl.G2);
     const int var = (er == 1 && eg == 1) ? 0 : ((er <= 2 && eg <= 2) ? 1 : ((er <= 4 && eg <= 2) ? 2 : 3));
-    {
-        // lean stage path of the kernel (wn_kernel.cuh crit_loop): one utterance, vectors that fill the 128-thread
-        // groups exactly, one gate quad / residual quad / skip quad per block, kernel_size 3, chunk-aligned exchanges
-        static const int evar[4][2] = {{1, 1}, {2, 2}, {4, 2}, {8, 8}};
-        const int chunk = 1 << pl.xc_shift;
-        pl.lean = (BT == 1 && (var == 1 || var == 2) && pl.ncopy == 1 && pl.kw == 3 && pl.RA == 4 && pl.NQ_A == 1 && pl.NQ_BO == 1 && pl.NQ_BS == 1 &&
-                   pl.NQ_D == 2 && pl.L >= 2 && evar[var][0] * 128 == pl.R && evar[var][1] * 128 == pl.G2 &&
-                   (evar[var][0] % 2) == 0 && (evar[var][1] % 2) == 0 && (pl.ex_yx % chunk) == 0 &&
-                   ((pl.G2 + pl.R) % chunk) == 0 && (pl.G2 % chunk) == 0 && (pl.xstride % 2) == 0 &&
-                   pl.S == pl.G2 && pl.NQ_HA == 1 && pl.NQ_HB == 1 && pl.O <= 128 && (pl.ex_sk % chunk) == 0 &&
-                   (pl.ex_h1 % chunk) == 0 &&
-                   env_int("WN_LEAN", 0) != 0) ? 1 : 0;
-    }
     const void* fn = nullptr;
     // stream launches take the STREAM instantiations (wn_kernel.cuh Engine); a stream holds at most one tile of 4
-#define WN_PICK(BT_, S_)                                                                      \
-    fn = var == 0 ? (const void*)wn::wn_persistent_kernel<BT_, 1, 1, false, S_>               \
-       : var == 1 ? (const void*)wn::wn_persistent_kernel<BT_, 2, 2, false, S_>               \
-       : var == 2 ? (const void*)wn::wn_persistent_kernel<BT_, 4, 2, false, S_>               \
-                  : (const void*)wn::wn_persistent_kernel<BT_, 8, 8, false, S_>
+#define WN_PICK(BT_, S_)                                                                \
+    fn = var == 0 ? (const void*)wn::wn_persistent_kernel<BT_, 1, 1, S_>               \
+       : var == 1 ? (const void*)wn::wn_persistent_kernel<BT_, 2, 2, S_>               \
+       : var == 2 ? (const void*)wn::wn_persistent_kernel<BT_, 4, 2, S_>               \
+                  : (const void*)wn::wn_persistent_kernel<BT_, 8, 8, S_>
     if (sc && BT > 4) return fail(WN_ERR_INVALID, "a stream holds at most 4 utterances");
     switch (BT) {
         case 1: if (sc) WN_PICK(1, true); else WN_PICK(1, false); break;
@@ -661,12 +649,7 @@ static int32_t launch_chunk(WnHandle* h, const wn_generate_args* a, int b0, int 
         default: WN_PICK(8, false); break;
     }
 #undef WN_PICK
-    if (pl.lean)      // the lean kernels: same plan, same packed weights, the lean stage path instead of the generic one
-        fn = sc ? (var == 1 ? (const void*)wn::wn_persistent_kernel<1, 2, 2, true, true>
-                            : (const void*)wn::wn_persistent_kernel<1, 4, 2, true, true>)
-                : (var == 1 ? (const void*)wn::wn_persistent_kernel<1, 2, 2, true>
-                            : (const void*)wn::wn_persistent_kernel<1, 4, 2, true>);
-    const int ai = (pl.lean ? 16 + var : bt_index(BT) * 4 + var) + (sc ? 20 : 0);
+    const int ai = bt_index(BT) * 4 + var + (sc ? 16 : 0);
     if (!h->attr_set[ai]) {
         CUDA_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_cap));
         h->attr_set[ai] = true;

@@ -86,7 +86,6 @@ struct WnPtrs {
     long long* prof;           // optional [P][8] cycle counters (scripts/sweep.py --prof)
     int warp_reverse;          // 1: logical warp = 9 - physical warp (the issue arbiter favours high warp ids)
     int gate_cycles;           // the critical group does not poll an exchange earlier than this after its own publish
-    int fast_gate;             // 1: approximate exponentials / division in the gate of the lean stage path
     // ---- streaming (wn_stream_generate): a launch continues an utterance at absolute step t_base
     unsigned t_base;           // absolute step of local step 0 (Philox counters, ring positions); 0 for a whole utterance
     float* state;              // NULL, or [P][ring floats] rings then the feedback [BT] s_in, [BT] s_idx, [BT][O] s_dense
@@ -175,8 +174,6 @@ __device__ __forceinline__ void st_pair(uint2* p, float v, uint32_t tag) {
     asm volatile("st.relaxed.gpu.global.v2.u32 [%0], {%1,%2};" ::"l"(p), "r"(__float_as_uint(v)), "r"(tag)
                  : "memory");
 }
-// acquire/release fence at block scope (__threadfence_block() is the sequentially-consistent one: MEMBAR.SC.CTA)
-__device__ __forceinline__ void fence_cta() { asm volatile("fence.acq_rel.cta;" ::: "memory"); }
 __device__ __forceinline__ int ld_flag(const int* p) {
     int v;
     asm volatile("ld.relaxed.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
@@ -319,48 +316,6 @@ __device__ __noinline__ bool wn_check_abort(volatile int* s_abort, int* err, lon
     return false;
 }
 
-// watchdog of the lean poll loops: no clock state on the stack, the elapsed time is bounded from below by the spin count
-// (a failed attempt is at least one L2 round trip, > 256 cycles)
-__device__ __noinline__ bool wn_poll_check(volatile int* s_abort, int* err, uint32_t spins, long long timeout,
-                                           uint32_t what, int p) {
-    if (*s_abort) return true;
-    if (ld_flag(err) != 0) {
-        *s_abort = 1;
-        return true;
-    }
-    if ((long long)spins * 256 > timeout) {
-        if (atomicCAS(err, 0, 1) == 0) {
-            err[1] = (int)what;
-            err[2] = p;
-            err[3] = (int)threadIdx.x;
-        }
-        *s_abort = 1;
-        return true;
-    }
-    return false;
-}
-// Slow paths of the lean stage code: the common case (barrier already complete / counter already reached) is one
-// inline test, everything else lives in these out-of-line loops so that the stage body stays short.
-__device__ __noinline__ bool wn_wait_bar_slow(uint64_t* bar, uint32_t parity, volatile int* s_abort, int* err,
-                                              long long timeout, uint32_t what, int p) {
-    uint32_t spins = 0;
-    long long t0 = 0;
-    while (!mbar_try_wait(bar, parity)) {
-        if (((++spins) & 255u) == 0 && wn_check_abort(s_abort, err, timeout, what, p, t0)) return false;
-    }
-    return true;
-}
-__device__ __noinline__ bool wn_wait_count_slow(volatile int* cnt, int need, unsigned sleep_ns, volatile int* s_abort,
-                                                int* err, long long timeout, uint32_t what, int p) {
-    uint32_t spins = 0;
-    long long t0 = 0;
-    while (*cnt < need) {
-        if (sleep_ns) __nanosleep(sleep_ns);
-        if (((++spins) & 63u) == 0 && wn_check_abort(s_abort, err, timeout, what, p, t0)) return false;
-    }
-    return true;
-}
-
 // ------------------------------------------------------------------------------------------
 #define WN_NTC 128                 // threads of one compute group (4 warps)
 #define WN_GW 4                    // warps per group
@@ -372,15 +327,11 @@ __device__ __noinline__ bool wn_wait_count_slow(volatile int* cnt, int need, uns
         default: { constexpr int E = 8; __VA_ARGS__ } break;  \
     }
 
-// LEAN: the lean stage path (crit_loop / def_loop) INSTEAD of the generic one -- a separate, smaller kernel: compiled
-// into the same kernel the two paths cost each other registers and instruction-cache footprint, which slows the
-// generic path with the lean code merely present.
 // STREAM: the kernel of wn_stream_generate (absolute steps, history and feedback in a state buffer).  A separate
 // instantiation too: any code after the step loops changes the register allocation of the loops (the config-2 kernel
 // then spills in its hot loop and loses 9 % on an H100 SXM at 400 W), so the whole-utterance kernels compile as before.
-template <int BT, int ER, int EG, bool LEAN = false, bool STREAM = false>
+template <int BT, int ER, int EG, bool STREAM = false>
 struct Engine {
-    static_assert(!LEAN || (BT == 1 && ER % 2 == 0 && EG % 2 == 0), "lean path: one utterance, paired elements");
     static constexpr int NV = 4 * BT;
     static constexpr int NA = (BT >= 8) ? 1 : 2;     // quads reduced together (their shuffle chains overlap)
     const WnPlan& pl;
@@ -651,34 +602,6 @@ struct Engine {
                 rs_par ^= 1u;
             }
         }
-    }
-
-    // lean variants (inline fast path, out-of-line spin)
-    __device__ __forceinline__ const float* acquire_lean(int t, int i) {
-        uint64_t* bar;
-        uint32_t par;
-        const float* ptr;
-        if (i < pl.nres) {
-            ptr = slots + (size_t)i * pl.slot_floats;
-            if (t != 0) return ptr;
-            bar = &bar_full[i];
-            par = 0;
-        } else {
-            const int slot = pl.nres + rs_slot;
-            ptr = slots + (size_t)slot * pl.slot_floats;
-            bar = &bar_full[slot];
-            par = rs_par;
-        }
-        if (!mbar_try_wait(bar, par)) {
-            if (!wn_wait_bar_slow(bar, par, s_abort, pp.err, pp.timeout_cycles, 0x80000000u | (uint32_t)i, p)) dead = true;
-        }
-        return ptr;
-    }
-    __device__ __forceinline__ void count_lean(volatile int* cnt, int need, unsigned sleep_ns, uint32_t what) {
-        if (*cnt < need) {
-            if (!wn_wait_count_slow(cnt, need, sleep_ns, s_abort, pp.err, pp.timeout_cycles, what, p)) dead = true;
-        }
-        fence_cta();
     }
 
     // ======================================================================================
@@ -985,23 +908,10 @@ struct Engine {
     // modules.py:154  tanh(a) * sigmoid(g) with a single division:
     //   (1 - e^{-2a}) / ((1 + e^{-2a}) (1 + e^{-g}));  |a| is clamped where tanh has saturated in fp32.
     // Absolute error ~1e-7 (the subtraction 1 - e^{-2a} loses relative, not absolute, accuracy near 0).
-    // ex2.approx / rcp.approx version (~1e-6 absolute error), selected at run time by pp.fast_gate
-    __device__ __forceinline__ static float gate_fast(float a, float g) {
-        const float ac = fminf(fmaxf(a, -15.0f), 15.0f);
-        const float ea = __expf(-2.0f * ac), eg = __expf(-g);
-        return __fdividef(1.0f - ea, (1.0f + ea) * (1.0f + eg));
-    }
     __device__ __forceinline__ static float gate(float a, float g) {
         const float ac = fminf(fmaxf(a, -15.0f), 15.0f);
-#ifdef WN_FAST_GATE
-        // ex2.approx based exponentials and an approximate division: ~2 ulp each, well inside the 1e-6
-        // absolute error the parity tests observe
-        const float ea = __expf(-2.0f * ac), eg = __expf(-g);
-        return __fdividef(1.0f - ea, (1.0f + ea) * (1.0f + eg));
-#else
         const float ea = expf(-2.0f * ac), eg = expf(-g);
         return (1.0f - ea) / ((1.0f + ea) * (1.0f + eg));
-#endif
     }
     // Everything of z_l(t) that does not depend on step t's broadcasts: (folded) bias + global conditioning
     // + local conditioning projection + the queued products of the older taps.  The deferred group builds
@@ -1075,123 +985,6 @@ struct Engine {
         long long t_pub = clock64();
         if (bar_groups(false)) return;      // the deferred group has built the pre-sums of step 0
 
-        // ---- lean stage path (pl.lean, set by wn_host.cu: one utterance, exact vector lengths, one gate quad and one
-        // residual quad per block).  A stage is a chain of dependent instructions executed by one warp per SM
-        // sub-partition, each waiting for the one before, so what a stage costs beyond the
-        // exchange is its LENGTH IN INSTRUCTIONS: same arithmetic as the generic loop below, with every address that
-        // does not depend on the stage computed once here, no per-element bounds checks, and the spin loops out of
-        // line.  One difference in order: a stage adds its x product (V x, formed while y is still travelling) to
-        // the accumulator before its y product (M y); the generic loop adds it after.  So the two paths agree to
-        // fp32 rounding, not bit for bit (tests/test_plan_variants.py).
-        constexpr bool LEAN_T = LEAN;
-        constexpr bool lean = LEAN;
-        constexpr int LY = LEAN_T ? EG / 2 : 1, LX = LEAN_T ? ER / 2 : 1;
-        long long lk_y[LY], lk_x[LX], l_inc = 0;
-        const uint2* l_in0 = xin;
-        uint2 *l_puby = pp.xbuf, *l_pubx = pp.xbuf;
-        const float* l_pre = pre;
-        const uint2 *l_sk0 = xin, *l_h10 = xin;
-        uint2 *l_pubs = pp.xbuf, *l_puba = pp.xbuf, *l_pubb = pp.xbuf;
-        int l_zy = 0, l_zx = 0, l_xo = 0, l_redw = 0, l_reda = 0, l_redx = 0, l_xb = 0, l_xs = 0;
-#pragma unroll
-        for (int j = 0; j < LY; ++j) lk_y[j] = 0;
-#pragma unroll
-        for (int j = 0; j < LX; ++j) lk_x[j] = 0;
-        if (lean) {
-#pragma unroll
-            for (int j = 0; j < LY; ++j) lk_y[j] = wn_pair_index((long long)(2 * gt + 2 * WN_NTC * j));
-#pragma unroll
-            for (int j = 0; j < LX; ++j) lk_x[j] = wn_pair_index((long long)(G2 + 2 * gt + 2 * WN_NTC * j));
-            l_inc = wn_pair_index((long long)YX);
-            l_in0 = xin + wn_pair_index((long long)pl.ex_yx);
-            l_puby = pp.xbuf + wn_pair_index((long long)pl.ex_yx) + wn_pair_index((long long)(y0 + max(it_y, 0)));
-            l_pubx = pp.xbuf + wn_pair_index((long long)pl.ex_yx) + wn_pair_index((long long)(G2 + x0r + max(it_x, 0)));
-            l_pre = pre + 2 * max(it_y, 0);
-            l_zy = pl.lb_Zy + 8 * gt;
-            l_zx = pl.lb_Zx + 8 * gt;
-            l_xo = pl.lb_Xo + 8 * gt;
-            l_redw = (lane >> 2) * WN_GW + gw;
-            l_reda = 2 * max(it_y, 0) * WN_GW;
-            l_redx = (4 + max(it_x, 0)) * WN_GW;
-            l_xb = pl.lb_xb + max(it_x, 0);
-            l_xs = x0r + max(it_x, 0);
-            l_sk0 = xin + wn_pair_index((long long)pl.ex_sk);
-            l_h10 = xin + wn_pair_index((long long)pl.ex_h1);
-            l_pubs = pp.xbuf + wn_pair_index((long long)(pl.ex_sk + s0 + max(it_s, 0)));
-            l_puba = pp.xbuf + wn_pair_index((long long)(pl.ex_h1 + a0 + max(it_a, 0)));
-            l_pubb = pp.xbuf + wn_pair_index((long long)(pl.ex_h2 + b0 + max(it_b, 0)));
-        }
-        // lean polls: the thread's pairs of the y part / the x part of one exchange, straight into registers.  A load
-        // whose two tags were good is not issued again (every attempt of every block lands on the same few L2 lines,
-        // and those reads are what the publishing stores queue behind)
-        auto lean_poll_y = [&](const uint2* base, uint32_t tag) {
-            uint4 ry[LY];
-            uint32_t need = (1u << LY) - 1u, spins = 0;
-            while (true) {
-#pragma unroll
-                for (int j = 0; j < LY; ++j)
-                    if (need & (1u << j)) ry[j] = ld_pair2(base + lk_y[j]);
-#pragma unroll
-                for (int j = 0; j < LY; ++j)
-                    if (((ry[j].y ^ tag) | (ry[j].w ^ tag)) == 0u) need &= ~(1u << j);
-                if (need == 0u) break;
-                if (((++spins) & 63u) == 0 && wn_poll_check(s_abort, pp.err, spins, pp.timeout_cycles, tag, p)) {
-                    dead = true;
-                    break;
-                }
-            }
-#pragma unroll
-            for (int j = 0; j < LY; ++j) {
-                yr[2 * j][0] = __uint_as_float(ry[j].x);
-                yr[2 * j + 1][0] = __uint_as_float(ry[j].z);
-            }
-        };
-        auto lean_poll_x = [&](const uint2* base, uint32_t tag) {
-            uint4 rx[LX];
-            uint32_t need = (1u << LX) - 1u, spins = 0;
-            while (true) {
-#pragma unroll
-                for (int j = 0; j < LX; ++j)
-                    if (need & (1u << j)) rx[j] = ld_pair2(base + lk_x[j]);
-#pragma unroll
-                for (int j = 0; j < LX; ++j)
-                    if (((rx[j].y ^ tag) | (rx[j].w ^ tag)) == 0u) need &= ~(1u << j);
-                if (need == 0u) break;
-                if (((++spins) & 63u) == 0 && wn_poll_check(s_abort, pp.err, spins, pp.timeout_cycles, tag | 0x40000000u, p)) {
-                    dead = true;
-                    break;
-                }
-            }
-#pragma unroll
-            for (int j = 0; j < LX; ++j) {
-                xr[2 * j][0] = __uint_as_float(rx[j].x);
-                xr[2 * j + 1][0] = __uint_as_float(rx[j].z);
-            }
-        };
-        // one row quad times the y-shaped / x-shaped register vector (wq already offset by the thread's 8*gt floats)
-        auto lean_quad_y = [&](const float* wq, float (&a4)[4]) {
-#pragma unroll
-            for (int j = 0; j < 2 * LY; ++j) {
-                const float4 a = *reinterpret_cast<const float4*>(wq + (2 * WN_NTC * (j >> 1) + (j & 1)) * 4);
-                const float v = yr[j][0];
-                a4[0] = fmaf(a.x, v, a4[0]); a4[1] = fmaf(a.y, v, a4[1]);
-                a4[2] = fmaf(a.z, v, a4[2]); a4[3] = fmaf(a.w, v, a4[3]);
-            }
-        };
-        auto lean_quad_x = [&](const float* wq, float (&a4)[4]) {
-#pragma unroll
-            for (int j = 0; j < 2 * LX; ++j) {
-                const float4 a = *reinterpret_cast<const float4*>(wq + (2 * WN_NTC * (j >> 1) + (j & 1)) * 4);
-                const float v = xr[j][0];
-                a4[0] = fmaf(a.x, v, a4[0]); a4[1] = fmaf(a.y, v, a4[1]);
-                a4[2] = fmaf(a.z, v, a4[2]); a4[3] = fmaf(a.w, v, a4[3]);
-            }
-        };
-        auto quad_sum = [](const float* r) {
-            const float4 q = *reinterpret_cast<const float4*>(r);
-            return (q.x + q.y) + (q.z + q.w);
-        };
-
         for (int t = 0; t < T; ++t) {
             const uint32_t tagbase = (uint32_t)t * NEID + 1u;
             if (prof) tc = clock64();
@@ -1200,26 +993,7 @@ struct Engine {
                 make_x0(xr);
                 WN_TICK(7);
                 // ------------------------------------------------------------ stage 0: layer 0 from x_0
-                if constexpr (LEAN_T) {
-                    {
-                        const float* W = acquire_lean(t, 0);
-                        const float pre_a = l_pre[0], pre_b = l_pre[1];
-                        float a4[4] = {0.f, 0.f, 0.f, 0.f};
-                        lean_quad_x(W + pl.fb_Zx + 8 * gt, a4);
-                        reduce_scatter<4>(a4, lane);
-                        if ((lane & 7) == 0) red1[(lane >> 3) * WN_GW + gw] = a4[0];
-                        WN_TICK(1);
-                        if (bar_or_n<1, WN_NTC>(dead)) { step_dead = true; break; }
-                        WN_TICK(2);
-                        if (it_y >= 0) {
-                            const float a = quad_sum(red1 + l_reda) + pre_a;
-                            const float g = quad_sum(red1 + l_reda + WN_GW) + pre_b;
-                            st_pair(l_puby, pp.fast_gate ? gate_fast(a, g) : gate(a, g), tagbase);
-                        }
-                        release_blob(t, 0);
-                        WN_TICK(3);
-                    }
-                } else {
+                {
                     const float* W = acquire_blob(t, 0);
                     float pre_a = 0.f, pre_b = 0.f;
                     if (it_y >= 0) { pre_a = pre[pa_idx]; pre_b = pre[pa_idx + BT]; }
@@ -1238,67 +1012,8 @@ struct Engine {
                     t_pub = clock64();
                     WN_TICK(3);
                 }
-                // ------------------------------------------------------------ stages 1..L-1, lean path
-                int s_next = 1;
-                if constexpr (LEAN_T) {
-                    if (lean) {
-                        s_next = L;
-                        for (int s = 1; s < L; ++s) {
-                            const float* W = acquire_lean(t, s);
-                            const float pre_a = l_pre[s * pl.RA4], pre_b = l_pre[s * pl.RA4 + 1];
-                            const uint32_t tag = tagbase + (uint32_t)(s - 1);
-                            const uint2* base = l_in0 + (long long)(s - 1) * l_inc;
-                            float* xst = xs + (s & 1) * R;
-                            float* yst = ys + (s & 1) * G2;
-                            // x_{s-1} was published by the DEFERRED groups half a stage ago (def_loop): normally one attempt,
-                            // and its product is formed while y_{s-1} is still travelling (x_0 is already in registers)
-                            if (s >= 2) lean_poll_x(base, tag);
-#pragma unroll
-                            for (int j = 0; j < LX; ++j)
-                                *reinterpret_cast<float2*>(xst + 2 * gt + 2 * WN_NTC * j) = make_float2(xr[2 * j][0], xr[2 * j + 1][0]);
-                            float a4[4] = {0.f, 0.f, 0.f, 0.f};
-                            lean_quad_x(W + l_zx, a4);
-                            float4 wy[2 * LY];          // weights of the y part: in registers before the data arrives
-#pragma unroll
-                            for (int j = 0; j < 2 * LY; ++j)
-                                wy[j] = *reinterpret_cast<const float4*>(W + l_zy + (2 * WN_NTC * (j >> 1) + (j & 1)) * 4);
-                            if (pp.gate_cycles > 0) { while (clock64() - t_pub < pp.gate_cycles) {} }
-                            WN_TICK(4);
-                            lean_poll_y(base, tag);
-                            WN_TICK(0);
-#pragma unroll
-                            for (int j = 0; j < 2 * LY; ++j) {
-                                const float yv = yr[j][0];
-                                a4[0] = fmaf(wy[j].x, yv, a4[0]); a4[1] = fmaf(wy[j].y, yv, a4[1]);
-                                a4[2] = fmaf(wy[j].z, yv, a4[2]); a4[3] = fmaf(wy[j].w, yv, a4[3]);
-                            }
-                            reduce_scatter<4>(a4, lane);
-                            float* r1 = red1 + (s & 1) * pl.red1_floats;
-                            if ((lane & 7) == 0) r1[(lane >> 3) * WN_GW + gw] = a4[0];
-#pragma unroll
-                            for (int j = 0; j < LY; ++j)
-                                *reinterpret_cast<float2*>(yst + 2 * gt + 2 * WN_NTC * j) = make_float2(yr[2 * j][0], yr[2 * j + 1][0]);
-                            if (bar_or_n<1, WN_NTC>(dead)) { step_dead = true; break; }
-                            if (gt == 0) {
-                                fence_cta();
-                                *s_stash_cnt = nstash + 1;
-                            }
-                            ++nstash;
-                            WN_TICK(1);
-                            if (it_y >= 0) {
-                                const float a = quad_sum(r1 + l_reda) + pre_a;
-                                const float g = quad_sum(r1 + l_reda + WN_GW) + pre_b;
-                                st_pair(l_puby + (long long)s * l_inc, pp.fast_gate ? gate_fast(a, g) : gate(a, g), tag + 1u);
-                            }
-                            release_blob(t, s);
-                            if (pp.gate_cycles > 0) t_pub = clock64();
-                            if (s >= 2) { count_lean(s_ddone_cnt, WN_GW * (ndone + 1), 0u, 0x08000000u); ++ndone; }
-                            WN_TICK(3);
-                        }
-                    }
-                }
                 // ------------------------------------------------------------ stages 1..L-1
-                for (int s = s_next; s < L; ++s) {
+                for (int s = 1; s < L; ++s) {
                     const float* W = acquire_blob(t, s);
                     float pre_a = 0.f, pre_b = 0.f;
                     if (it_y >= 0) { pre_a = pre[pa_idx + s * pl.RA4 * BT]; pre_b = pre[pa_idx + s * pl.RA4 * BT + BT]; }
@@ -1363,68 +1078,6 @@ struct Engine {
                     WN_TICK(3);
                 }
                 if (step_dead) break;
-                bool tail_done = false;
-                if constexpr (LEAN_T) {
-                    if (lean) {
-                        // ---- lean stage L, head 1, head 2 (same arithmetic as the generic code below)
-                        tail_done = true;
-                        const float* H = acquire_lean(t, L);
-                        lean_poll_x(l_in0 + (long long)(L - 1) * l_inc, tagbase + (uint32_t)(L - 1));
-                        lean_poll_y(l_in0 + (long long)(L - 1) * l_inc, tagbase + (uint32_t)(L - 1));
-                        WN_TICK(0);
-                        float* xst = xs + (L & 1) * R;
-#pragma unroll
-                        for (int j = 0; j < LX; ++j)
-                            *reinterpret_cast<float2*>(xst + 2 * gt + 2 * WN_NTC * j) = make_float2(xr[2 * j][0], xr[2 * j + 1][0]);
-                        float* r1 = red1 + (L & 1) * pl.red1_floats;
-                        float* r1a = red1 + ((L + 1) & 1) * pl.red1_floats;
-                        {
-                            float a4[4] = {0.f, 0.f, 0.f, 0.f};
-                            lean_quad_y(H + pl.tb_Sk + 8 * gt, a4);
-                            reduce_scatter<4>(a4, lane);
-                            if ((lane & 7) == 0) r1[(lane >> 3) * WN_GW + gw] = a4[0];
-                        }
-                        WN_TICK(1);
-                        if (bar_or_n<1, WN_NTC>(dead)) { step_dead = true; break; }
-                        if (gt == 0) {
-                            fence_cta();
-                            *s_stash_cnt = nstash + 1;
-                        }
-                        ++nstash;
-                        // skip rows of layers 0..L-2 were accumulated by the deferred group: wait for its stage L-1
-                        count_lean(s_ddone_cnt, WN_GW * (ndone + 1), 0u, 0x08000001u);
-                        ++ndone;
-                        WN_TICK(2);
-                        if (it_s >= 0) {
-                            float tot = quad_sum(r1 + it_s * WN_GW) + H[pl.tb_sb + it_s];
-                            tot = skipacc[it_s] + tot;
-                            st_pair(l_pubs, fmaxf(tot * pl.skip_scale, 0.f), tagbase + (uint32_t)L);
-                        }
-                        WN_TICK(3);
-                        if (na > 0) {
-                            lean_poll_y(l_sk0, tagbase + (uint32_t)L);
-                            float a4[4] = {0.f, 0.f, 0.f, 0.f};
-                            lean_quad_y(H + pl.tb_Ha + 8 * gt, a4);
-                            reduce_scatter<4>(a4, lane);
-                            if ((lane & 7) == 0) r1a[(lane >> 3) * WN_GW + gw] = a4[0];
-                        }
-                        if (bar_or_n<1, WN_NTC>(dead)) { step_dead = true; break; }
-                        if (it_a >= 0)
-                            st_pair(l_puba, fmaxf(quad_sum(r1a + it_a * WN_GW) + H[pl.tb_Hab + it_a], 0.f), tagbase + (uint32_t)L + 1u);
-                        if (nb > 0) {
-                            lean_poll_y(l_h10, tagbase + (uint32_t)L + 1u);
-                            float a4[4] = {0.f, 0.f, 0.f, 0.f};
-                            lean_quad_y(H + pl.tb_Hb + 8 * gt, a4);
-                            reduce_scatter<4>(a4, lane);
-                            if ((lane & 7) == 0) r1[(lane >> 3) * WN_GW + gw] = a4[0];
-                        }
-                        if (bar_or_n<1, WN_NTC>(dead)) { step_dead = true; break; }
-                        if (it_b >= 0)
-                            st_pair(l_pubb, quad_sum(r1 + it_b * WN_GW) + H[pl.tb_Hbb + it_b], tagbase + (uint32_t)L + 2u);
-                        release_blob(t, L);
-                    }
-                }
-                if (!tail_done) {
                 // ------------------------------------------------------------ stage L: skip of the last layer
                 const float* H = acquire_blob(t, L);
                 {
@@ -1478,7 +1131,6 @@ struct Engine {
                     publish(pl.ex_h2 + b0 + fr, fb, cp_b, red_sum(r1, fr, fb) + H[pl.tb_Hbb + fr], tagbase + wn_eid_h2(pl));
                 }
                 release_blob(t, L);
-                }
                 {
                     WN_DISPATCH_E(EO, { float h[E][BT];
                                         poll_vec<E>(xin, pl.ex_h2, O, tagbase + wn_eid_h2(pl), h);
@@ -1541,130 +1193,9 @@ struct Engine {
 #define WN_TICK(i) if (prof) { const long long now_ = clock64(); pc[i] += now_ - tc; tc = now_; }
         int nstash = 0;
 
-        // lean variant of a deferred stage (see crit_loop): two older-tap quads (acc[0..7]) + one skip quad (accs)
-        constexpr bool LEAN_T = LEAN;
-        constexpr bool lean = LEAN;
-        const int d_tap = (gt < nring_items) ? gt / pl.RA : 0, d_rr = (gt < nring_items) ? gt % pl.RA : 0;
-        // the residual stream is published from here (threads 64.. of the group), half a stage before the critical
-        // group of any block asks for it: its poll then spins on y alone (a third of the exchange)
-        int d_x0r, d_nx;
-        wn_part(R, P, p, d_x0r, d_nx);
-        const int d_fx = (gt >= 64 && gt < 64 + d_nx) ? gt - 64 : -1;
-        uint2* d_pubx = pp.xbuf;
-        long long d_inc = 0;
-        if (lean) {
-            d_pubx = pp.xbuf + wn_pair_index((long long)pl.ex_yx) + wn_pair_index((long long)(G2 + d_x0r + max(d_fx, 0)));
-            d_inc = wn_pair_index((long long)(G2 + R));
-        }
-        const float RSQRT2 = 0.70710678118654752440f;         // math.sqrt(0.5), modules.py:162
-        auto lean_stage = [&](int t, int s, int layer, const float* Td, const float* Sk, const float* skb) -> bool {
-            count_lean(s_stash_cnt, nstash + 1, 32u, 0x04000000u);
-            ++nstash;
-            WN_TICK(0);
-            const float* xst = xs + (s & 1) * R;
-            const float* yst = ys + (s & 1) * G2;
-            float* red = red2 + (s & 1) * pl.red2_floats;
-            // ---- phase 1: the block's rows of x_s, published at once (the critical groups of all blocks need them
-            // for stage s+1, before anything else this group produces)
-            // rows of x_s = (conv1x1_out_{s-1} y_{s-1} + b + x_{s-1}) sqrt(.5)  (modules.py:160-162), not in the tail stage
-            float accx[4] = {0.f, 0.f, 0.f, 0.f};
-            const float* Wb = Sk ? Sk - pl.lb_Sk : nullptr;     // the blob of stage s
-            if (Sk) {
-                const float* wx = Wb + pl.lb_Xo + 8 * gt;
-#pragma unroll
-                for (int j = 0; j < EG / 2; ++j) {
-                    const float2 yv2 = *reinterpret_cast<const float2*>(yst + 2 * gt + 2 * WN_NTC * j);
-#pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        const float4 a = *reinterpret_cast<const float4*>(wx + (2 * WN_NTC * j + h) * 4);
-                        const float yv = h ? yv2.y : yv2.x;
-                        accx[0] = fmaf(a.x, yv, accx[0]); accx[1] = fmaf(a.y, yv, accx[1]);
-                        accx[2] = fmaf(a.z, yv, accx[2]); accx[3] = fmaf(a.w, yv, accx[3]);
-                    }
-                }
-            }
-            if (Sk) {
-                reduce_scatter<4>(accx, lane);
-                if ((lane & 7) == 0) red[(12 + (lane >> 3)) * WN_GW + gw] = accx[0];
-                if (bar_or_n<2, WN_NTC>(dead)) dead = true;
-                if (!dead && d_fx >= 0) {
-                    const float4 q = *reinterpret_cast<const float4*>(red + (12 + d_fx) * WN_GW);
-                    const float o = ((q.x + q.y) + (q.z + q.w)) + Wb[pl.lb_xb + d_fx];
-                    st_pair(d_pubx + (long long)s * d_inc, (o + xst[d_x0r + d_fx]) * RSQRT2,
-                            (uint32_t)t * ((uint32_t)L + 3u) + 1u + (uint32_t)s);
-                }
-            }
-            // ---- phase 2: queued older-tap products and skip rows
-            float acc[8], accs[4];
-#pragma unroll
-            for (int v = 0; v < 8; ++v) acc[v] = 0.f;
-#pragma unroll
-            for (int v = 0; v < 4; ++v) accs[v] = 0.f;
-            {
-                const float *w0 = Td + 8 * gt, *w1 = Td + (size_t)R * 4 + 8 * gt;
-#pragma unroll
-                for (int j = 0; j < ER / 2; ++j) {
-                    const float2 xv2 = *reinterpret_cast<const float2*>(xst + 2 * gt + 2 * WN_NTC * j);
-#pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        const int ko = (2 * WN_NTC * j + h) * 4;
-                        const float4 a = *reinterpret_cast<const float4*>(w0 + ko);
-                        const float4 b = *reinterpret_cast<const float4*>(w1 + ko);
-                        const float xv = h ? xv2.y : xv2.x;
-                        acc[0] = fmaf(a.x, xv, acc[0]); acc[1] = fmaf(a.y, xv, acc[1]);
-                        acc[2] = fmaf(a.z, xv, acc[2]); acc[3] = fmaf(a.w, xv, acc[3]);
-                        acc[4] = fmaf(b.x, xv, acc[4]); acc[5] = fmaf(b.y, xv, acc[5]);
-                        acc[6] = fmaf(b.z, xv, acc[6]); acc[7] = fmaf(b.w, xv, acc[7]);
-                    }
-                }
-            }
-            if (Sk) {
-                const float* ws = Sk + 8 * gt;
-#pragma unroll
-                for (int j = 0; j < EG / 2; ++j) {
-                    const float2 yv2 = *reinterpret_cast<const float2*>(yst + 2 * gt + 2 * WN_NTC * j);
-#pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        const float4 a = *reinterpret_cast<const float4*>(ws + (2 * WN_NTC * j + h) * 4);
-                        const float yv = h ? yv2.y : yv2.x;
-                        accs[0] = fmaf(a.x, yv, accs[0]); accs[1] = fmaf(a.y, yv, accs[1]);
-                        accs[2] = fmaf(a.z, yv, accs[2]); accs[3] = fmaf(a.w, yv, accs[3]);
-                    }
-                }
-            }
-            reduce_scatter<8>(acc, lane);
-            reduce_scatter<4>(accs, lane);
-            if ((lane & 3) == 0) red[(lane >> 2) * WN_GW + gw] = acc[0];
-            if (Sk != nullptr && (lane & 7) == 0) red[(8 + (lane >> 3)) * WN_GW + gw] = accs[0];
-            WN_TICK(1);
-            const bool d = bar_or_n<2, WN_NTC>(dead);
-            if (!d) {
-
-                if (gt < nring_items) {
-                    const int e = (layer * (kw - 1) + d_tap) * 3;
-                    const float4 q = *reinterpret_cast<const float4*>(red + gt * WN_GW);
-                    ring[((size_t)ringtab[e] + ringtab[e + 2]) * pl.RA4 + d_rr] = (q.x + q.y) + (q.z + q.w);
-                }
-                if (Sk != nullptr && gt >= 32 && gt < 32 + nskip_items) {
-                    const int f = gt - 32;
-                    const float4 q = *reinterpret_cast<const float4*>(red + (8 + f) * WN_GW);
-                    const float h = ((q.x + q.y) + (q.z + q.w)) + skb[f];
-                    skipacc[f] = (layer == 0) ? h : skipacc[f] + h;
-                }
-            }
-            fence_cta();
-            __syncwarp();
-            if (lane == 0) atomicAdd((int*)s_ddone_cnt, 1);
-            WN_TICK(2);
-            return d;
-        };
-
         // one deferred stage: `Td` = older taps of `layer` (uses x), `Sk`/`skb` = skip rows of `layer`
         // (uses y; nullptr in the tail stage, where the critical group evaluates them itself)
         auto stage = [&](int t, int s, int layer, const float* Td, const float* Sk, const float* skb) {
-            if constexpr (LEAN_T) {
-                if (lean) return lean_stage(t, s, layer, Td, Sk, skb);
-            }
             wait_count<true>(s_stash_cnt, nstash + 1, 0x04000000u);
             ++nstash;
             WN_TICK(0);
@@ -1778,11 +1309,11 @@ __device__ __noinline__ void wn_store_state(const WnPlan& pl, const WnPtrs& pp, 
 // ------------------------------------------------------------------------------------------
 // kernel entry
 // ------------------------------------------------------------------------------------------
-template <int BT, int ER, int EG, bool LEAN = false, bool STREAM = false>
+template <int BT, int ER, int EG, bool STREAM = false>
 __global__ void __launch_bounds__(WN_NTHREADS, 1)
 wn_persistent_kernel(const __grid_constant__ WnPlan pl, const __grid_constant__ WnPtrs pp) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
-    Engine<BT, ER, EG, LEAN, STREAM> eng(pl, pp, smem_raw);
+    Engine<BT, ER, EG, STREAM> eng(pl, pp, smem_raw);
     const int tid = eng.tid, p = blockIdx.x;      // logical thread index (see Engine)
     const int nslots = pl.nres + pl.nring;
     if (tid == 0) {

@@ -83,7 +83,6 @@ struct WnPlan {
     int red2_floats;            // one of the two deferred-partials buffers
     float skip_scale;           // sqrt(1/L), wavenet.py:313
     int xc_shift, xstride;      // exchange layout: 2^xc_shift pairs per chunk, chunks xstride pairs apart
-    int lean;                   // 1: the kernel may take its lean stage path (wn_host.cu launch_chunk decides)
 };
 WN_HD long long wn_pair_index_(const WnPlan& pl, long long lin) {
     return (long long)(((unsigned long long)lin >> pl.xc_shift) * (unsigned long long)pl.xstride +
