@@ -42,6 +42,11 @@ NLL_CASES = {
     "gauss_o2": ("gauss", 2, 65536, -7.0),
     "gauss_o9": ("gauss", 9, 65536, -16.0),
     "softmax_o256": ("softmax", 256, 256, -16.0),
+    # appended (each case's seed is its position): the C == 3 Gaussian (mean y[1], log-scale y[2], no mixture
+    # weights), a one-component MoL, and an odd number of classes
+    "gauss_o3": ("gauss", 3, 65536, -7.0),
+    "mol_o3": ("mol", 3, 256, -16.0),
+    "softmax_o255": ("softmax", 255, 255, -16.0),
 }
 NLL_B, NLL_T = 2, 96
 Y_EDGE, Y_MARGIN, DELTA_MARGIN = 0.999, 1e-4, 0.1    # |y| - 0.999 and cdf_delta / 1e-5 - 1 stay this far from 0

@@ -27,6 +27,8 @@ BASES = {
     "cfg5": dict(kw=FULL["cfg5_mol30"]["kw"], T=2100, T_tf=256),
     # gate half 640, variant <8, 8>: at a tile of 2 or 4 every blob streams through two slots
     "eg8": dict(kw=dict(full_kw("eg8")), T=96),
+    # ragged: kernel size 7, 81 conditioning channels, 33 MoL head rows; largest ring delay 48
+    "mol_k11": dict(kw=dict(full_kw("mol_k11")), T=112),
 }
 for _b in BASES.values():
     _b["kw"] = dict(_b["kw"], dropout=0.0)
@@ -36,7 +38,7 @@ for _b in BASES.values():
     _b.setdefault("T_tf", _b["T"])
 
 # head-output bound against float64 forward(): test_forward.py / shape_cases.py's, 1e-4 for the 512-wide stacks
-TOL64 = {"cfg1": 2e-5, "cfg2": 1e-4, "cfg3": 2e-5, "cfg5": 1e-4, "eg8": 1e-4}
+TOL64 = {"cfg1": 2e-5, "cfg2": 1e-4, "cfg3": 2e-5, "cfg5": 1e-4, "eg8": 1e-4, "mol_k11": 2e-5}
 
 # a stream is cut into chunks of 1, 7 and 64 samples, then the rest
 STREAM_SPLIT = (1, 7, 64)
@@ -141,6 +143,12 @@ MATRIX = [
     _e("eg8_b2_warp_reverse", "eg8", B=2, env={"WN_WARP_REVERSE": 1}, expect=dict(batch_tile=2, resident_blobs=3),
        stream=True),
     _e("eg8_tile8", "eg8", B=8, env={"WN_MAX_TILE": 8}, expect=dict(batch_tile=8)),
+
+    # ---------------- engine 5, ragged rows: 7 blocks divide none of the vectors.  Each block is sized for 4 gate
+    # pairs (RA = 8), 3 residual, 4 skip and 5 head rows; gate 26 = 5 x 4 + 2 x 3, residual 18 = 4 x 3 + 3 x 2,
+    # skip 22 = 4 + 6 x 3, head 33 = 5 x 5 + 2 x 4
+    _e("mol_k11_ctas7", "mol_k11", env={"WN_NUM_CTAS": 7},
+       expect=dict(num_ctas=7, rows_y=4, rows_x=3, rows_skip=4, rows_head_b=5), bit=NUM_CTAS_WHY),
 
     # ---------------- engine 5, softmax head: replicas, layout, warp order
     _e("cfg1_ncopy4_env", "cfg1", env={"WN_NCOPY": 4}, expect=dict(exchange_copies=4, resident_blobs=13)),
@@ -252,9 +260,9 @@ def max_tile(env, engine):
 
 def make_module(base):
     """The seeded CPU module of a base shape (eval mode), built as full_case / shape_cases.make_module build it."""
-    if base == "eg8":
+    if base in ("eg8", "mol_k11"):
         from shape_cases import make_module as shape_module
-        return shape_module("eg8")
+        return shape_module(base)
     from test_gpu_parity import full_case
     name = {"cfg1": "cfg1_mulaw256", "cfg2": "cfg2_mol24", "cfg3": "cfg3_gauss_spk", "cfg5": "cfg5_mol30"}[base]
     return full_case(name)[0]

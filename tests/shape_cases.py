@@ -1,7 +1,9 @@
 # coding: utf-8
 """Model shapes the planner accepts beyond the golden cases and the BASELINE configurations: kernel sizes 1, 2, 4 and
 8, one layer, one-layer stacks, gate halves above 512, residual / skip vectors of 1024, 128 conditioning channels, a
-MoL head of 34 mixtures and a softmax head of 1024 classes.  Shared by tests/test_shape_coverage_host.py (planner,
+MoL head of 34 mixtures and a softmax head of 1024 classes; and ragged shapes -- vectors of 2 mod 4 that the block
+count does not divide, heads of 3 channels (a Gaussian and a one-component MoL) and of 33 and 255 rows, kernel sizes
+5, 6 and 7, conditioning widths of 1, 3 and 81.  Shared by tests/test_shape_coverage_host.py (planner,
 packer and oracle without a GPU) and tests/test_shape_coverage.py (the kernel on an H100).
 
 Every case is a seeded ``WaveNet`` with biases drawn from N(0, 0.05) (the reference initialises them to zero, so bias
@@ -46,6 +48,26 @@ CASES = {
     # 1024 classes: the widest second head stage, the one-hot gather and the dense softmax feedback
     "softmax_wide": dict(kernel_size=3, layers=4, stacks=2, residual_channels=64, gate_channels=128,
                          skip_out_channels=256, out_channels=1024, scalar_input=False),
+    # ---- ragged shapes: residual, gate half and skip of 2 mod 4, odd heads, odd conditioning widths.  n rows over P
+    # blocks are split n % P blocks of ceil(n / P) rows and the rest one row fewer (wn_plan.h wn_part), so a vector
+    # that P does not divide leaves some blocks' row quads partly filled, or the blocks past n with no rows at all
+    # a Gaussian head of 3 channels (mean y[1], log-scale y[2]); kernel size 5 (8 older-tap rows in 2 quads);
+    # 6 blocks: 4 own 2 skip rows and 2 own one, 3 own a head row and 3 none
+    "gauss3_r6": dict(kernel_size=5, layers=6, stacks=2, residual_channels=6, gate_channels=12, skip_out_channels=10,
+                      out_channels=3, scalar_input=True, output_distribution="Normal", cin_channels=3),
+    # a one-component MoL: the Gumbel argmax over one logit and a loss mixture of one term; one conditioning channel;
+    # 10 blocks: 4 own 2 skip rows and 6 own one, 3 own a head row and 7 none
+    "mol_k1": dict(kernel_size=3, layers=4, stacks=2, residual_channels=10, gate_channels=20, skip_out_channels=14,
+                   out_channels=3, scalar_input=True, output_distribution="Logistic", cin_channels=1),
+    # kernel size 7 (12 older-tap rows in 3 quads); 81 conditioning channels (a third group, partly filled and odd);
+    # 26 blocks: 18 own a residual row and 8 none, 22 own a skip row and 4 none, 7 own 2 head rows and 19 one
+    "mol_k11": dict(kernel_size=7, layers=8, stacks=2, residual_channels=18, gate_channels=52, skip_out_channels=22,
+                    out_channels=33, scalar_input=True, output_distribution="Logistic", cin_channels=81),
+    # 255 classes: the odd tail of the paired exchange poll at a tile of 1 (2 elements per thread); kernel size 6
+    # (10 older-tap rows, the third quad half filled); stacks of 2 layers; 18 blocks: 3 own 15 head rows and 15 own
+    # 14, residual 8 x 2 + 10 x 1, skip 12 x 2 + 6 x 1; 60 items at a tile of 4, just under the 64 limit
+    "softmax_255": dict(kernel_size=6, layers=6, stacks=3, residual_channels=26, gate_channels=36,
+                        skip_out_channels=30, out_channels=255, scalar_input=False),
 }
 NAMES = list(CASES)
 

@@ -6,7 +6,8 @@
   - against the engine's own fully teacher-forced wn_generate (config 5 at T = 240 000 included);
   - bit identity: a repeat call, row b of a batch against the utterance alone, class ids against dense one-hot rows,
     conditioning frames against the sample-rate conditioning the engine's upsampler makes;
-  - softmax=True, wn_nll against tests/golden/nll.npz, WaveNet.nll against the oracle criterion, and the refusals."""
+  - softmax=True, wn_nll against tests/golden/nll.npz, WaveNet.nll against the oracle criterion (golden cases and the
+    3-channel and 255-class shape cases), and the refusals."""
 import ctypes as C
 
 import pytest
@@ -179,6 +180,28 @@ def test_module_nll_against_oracle_criterion(name, kind):
         print("%s %s: nll %.6f, float64 oracle %.6f" % (name, kwargs, got, want))
         assert abs(got - want) <= 1e-4 * max(1.0, abs(want)), (got, want)
     per = m.nll(x, c=c, g=g, num_classes=256, log_scale_min=-7.0, reduce=False).cpu()
+    want = lo.criterion(kind, head64, target, num_classes=256, log_scale_min=-7.0, reduce=False)
+    assert per.shape == (B, T - 1)
+    assert float(((per.double() - want).abs() / want.abs().clamp(min=1.0)).max()) <= 1e-3
+
+
+@pytest.mark.parametrize("name,kind", [("gauss3_r6", "gauss"), ("mol_k1", "mol"), ("softmax_255", "softmax")])
+def test_module_nll_on_shape_cases_against_oracle_criterion(name, kind):
+    """The C == 3 Gaussian, a one-component MoL and 255 classes, end to end: the dense forward on a ragged shape,
+    then wn_nll, against the oracle criterion on float64 forward()."""
+    sc = ShapeCase(name, B=2, T=96, oracle=False)
+    m = fresh_module(sc.kw, sc.sd).cuda()
+    x, c = sc.x_tf, sc.t("c_up")
+    head64 = sc.forward64()
+    target = x[:, 0, :].double() if sc.cfg.scalar_input else x.argmax(1)
+    B, T = target.shape
+    lengths = torch.tensor([T, T - 9])
+    for kwargs in (dict(), dict(lengths=lengths)):
+        want = float(lo.criterion(kind, head64, target, num_classes=256, log_scale_min=-7.0, **kwargs))
+        got = float(m.nll(x, c=c, num_classes=256, log_scale_min=-7.0, **kwargs))
+        print("%s %s: nll %.6f, float64 oracle %.6f" % (name, kwargs, got, want))
+        assert abs(got - want) <= 1e-4 * max(1.0, abs(want)), (got, want)
+    per = m.nll(x, c=c, num_classes=256, log_scale_min=-7.0, reduce=False).cpu()
     want = lo.criterion(kind, head64, target, num_classes=256, log_scale_min=-7.0, reduce=False)
     assert per.shape == (B, T - 1)
     assert float(((per.double() - want).abs() / want.abs().clamp(min=1.0)).max()) <= 1e-3

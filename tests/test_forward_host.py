@@ -2,8 +2,8 @@
 """Teacher-forced scoring without a GPU:
   - oracle/loss_oracle.py equals the unmodified reference's per-sample losses stored in tests/golden/nll.npz, on every
     branch (cdf_delta on both sides of 1e-5 at 256 and 65536 classes, targets beyond +-0.999, clamped log-scales,
-    Gaussian heads of 2 and 3K channels, a softmax head of 256 classes);
-  - wn_nll refuses malformed arguments before it touches the device;
+    Gaussian heads of 2, 3 and 3K channels, a one-component MoL head, softmax heads of 255 and 256 classes);
+  - wn_nll and the stand-alone samplers refuse malformed arguments before they touch the device;
   - the library exports wn_forward and wn_nll, still reports ABI 3 and seven structs, and carries sm_90a code."""
 import ctypes as C
 import os
@@ -61,7 +61,12 @@ def test_golden_losses_reach_every_branch():
         seen["edge_lo"] += int((y < -0.999).sum())
         seen["clamped"] += int((y_hat[:, 2 * K:] < cs["log_scale_min"]).sum())
     assert all(v > 0 for v in seen.values()), seen
-    assert {nll_case(n)["y_hat"].size(1) for n in nll_cases() if nll_case(n)["head"] == "gauss"} >= {2, 9}
+    widths = {}
+    for n in nll_cases():
+        cs = nll_case(n)
+        widths.setdefault(cs["head"], set()).add(cs["y_hat"].size(1))
+    # a single Gaussian of 2 and of 3 channels, a one-component MoL, and an odd number of classes
+    assert widths["gauss"] >= {2, 3, 9} and 3 in widths["mol"] and 255 in widths["softmax"], widths
 
 
 def test_oracle_criterion_masks_as_train_py():
@@ -101,6 +106,15 @@ def test_wn_nll_refuses_malformed_arguments(kw, msg):
     rc = nll_status(**kw)
     assert rc == -1, rc
     assert msg in N.lib().wn_last_error().decode(), N.lib().wn_last_error()
+
+
+@pytest.mark.parametrize("fn", ["wn_sample_mol", "wn_sample_gauss"])
+@pytest.mark.parametrize("B,O,T", [(0, 3, 8), (2, 3, 0), (2, 0, 8), (-1, 3, 8), (2, -3, 8), (2, 3, -8)])
+def test_samplers_refuse_empty_shapes(fn, B, O, T):
+    """O = 0 passes the O % 3 check: without the shape check the kernel would read an empty head."""
+    rc = getattr(N.lib(), fn)(FAKE, B, O, T, FAKE, FAKE, FAKE, None)
+    assert rc == -1, rc
+    assert "%s: B, O and T must be >= 1" % fn in N.lib().wn_last_error().decode(), N.lib().wn_last_error()
 
 
 def test_forward_entry_points_without_an_abi_bump():

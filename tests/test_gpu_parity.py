@@ -242,26 +242,41 @@ def test_philox_sampling_is_seed_reproducible_and_self_consistent():
     assert y4.shape == y1.shape
 
 
-def test_standalone_samplers_match_oracle():
+def check_standalone_samplers(K, B, T):
+    """The stand-alone MoL and Gaussian samplers on seeded (B, 3K, T) head outputs, and the single Gaussian on the
+    first two channels, against the oracle's samplers on the same replayed noise."""
     from wavenet_vocoder_b200.mixture import sample_from_discretized_mix_logistic, sample_from_mix_gaussian
     gen = torch.Generator().manual_seed(3)
-    B, K, T = 3, 10, 50
     y = torch.randn(B, 3 * K, T, generator=gen)
     y[:, 2 * K:] -= 2.0
     u1 = torch.empty(T, B, K).uniform_(1e-5, 1 - 1e-5, generator=gen)
     u2 = torch.empty(T, B).uniform_(1e-5, 1 - 1e-5, generator=gen)
     z = torch.randn(T, B, generator=gen)
     got = sample_from_discretized_mix_logistic(y.cuda(), noise={"u1": u1, "u2": u2}).cpu()
-    got_g = sample_from_mix_gaussian(y.cuda(), noise={"u1": u1, "z": z}).cpu()
+    # a single Gaussian of 3 channels draws no mixture indicator: the wrapper passes no u1
+    got_g = sample_from_mix_gaussian(y.cuda(), noise={"u1": u1, "z": z} if K > 1 else {"z": z}).cpu()
     got_1 = sample_from_mix_gaussian(y[:, :2].contiguous().cuda(), noise={"z": z}).cpu()
+    assert got.shape == got_g.shape == got_1.shape == (B, T)
     for t in range(T):
         yt = y[:, :, t].unsqueeze(1)
         ref = orc.sample_mol(yt, orc.ReplayNoise(uniform=[u1[t].unsqueeze(1), u2[t].unsqueeze(1)]))
         assert float((got[:, t:t + 1] - ref).abs().max()) <= 1e-5
-        ref_g = orc.sample_gaussian(yt, orc.ReplayNoise(uniform=[u1[t].unsqueeze(1)], normal=[z[t].unsqueeze(1)]))
+        ref_g = orc.sample_gaussian(yt, orc.ReplayNoise(uniform=[u1[t].unsqueeze(1)] if K > 1 else [],
+                                                        normal=[z[t].unsqueeze(1)]))
         assert float((got_g[:, t:t + 1] - ref_g).abs().max()) <= 1e-5
         ref_1 = orc.sample_gaussian(yt[:, :, :2], orc.ReplayNoise(normal=[z[t].unsqueeze(1)]))
         assert float((got_1[:, t:t + 1] - ref_1).abs().max()) <= 1e-5
+
+
+def test_standalone_samplers_match_oracle():
+    check_standalone_samplers(10, 3, 50)
+
+
+# K = 1: a one-component MoL and the C == 3 Gaussian (mean y[1], log-scale y[2]); B x T = 771 leaves the last
+# 256-thread block of the sampler kernel ragged
+@pytest.mark.parametrize("K,B,T", [(1, 3, 50), (10, 3, 257), (1, 3, 257)])
+def test_standalone_samplers_at_more_widths_match_oracle(K, B, T):
+    check_standalone_samplers(K, B, T)
 
 
 # ------------------------------------------------------------------------------------------------

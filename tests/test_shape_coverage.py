@@ -1,6 +1,7 @@
 # coding: utf-8
 """The kernels on the model shapes of tests/shape_cases.py (kernel sizes 1, 2, 4 and 8, one layer, one-layer stacks,
-a gate half of 640, residual / skip vectors of 1024, 128 conditioning channels, 34 mixtures, 1024 classes), on an H100:
+a gate half of 640, residual / skip vectors of 1024, 128 conditioning channels, 34 mixtures, 1024 classes, and the
+ragged shapes: vectors of 2 mod 4, heads of 3, 33 and 255, kernel sizes 5 to 7), on an H100:
   - teacher-forced head outputs against the fp32 oracle and against the module's float64 batch forward();
   - free running under replayed noise against the oracle (waveform RMS; class ids on the kernel's own trajectory);
   - streams: chunked == one shot bit for bit, chunk boundaries at different ring phases;
@@ -15,6 +16,7 @@ from oracle import wavenet_oracle as orc
 from helpers import GoldenCase
 from shape_cases import MAX_B, NAMES, PARAM_TOL, ShapeCase, fresh_module, full_kw, max_delay, path_config
 from test_gpu_parity import RMS_TOL, assert_class_ids_match
+from test_shape_coverage_host import cfg_of, plan_status
 from test_streaming import assert_same, chunked, inputs_for, model_of, one_shot
 from test_upsample import TOL as UPS_TOL, model_for
 
@@ -23,8 +25,16 @@ pytestmark = pytest.mark.gpu
 
 @pytest.fixture(params=[5, 7])
 def engine(request, monkeypatch):
-    """Both kernel organisations: 5 = the default (csrc/wn_kernel.cuh), 7 = the alternative (csrc/wn7_kernel.cuh)."""
+    """Both kernel organisations: 5 = the default (csrc/wn_kernel.cuh), 7 = the alternative (csrc/wn7_kernel.cuh).
+    A case engine 7 does not plan at the test's batch is skipped for engine 7 with the planner's message."""
     monkeypatch.setenv("WN_ENGINE", str(request.param))
+    params = getattr(request.node, "callspec", None)
+    name = params.params.get("name") if params is not None else None
+    if request.param == 7 and name is not None:
+        B = params.params.get("B", MAX_B[name])
+        rc, msg = plan_status(cfg_of(name), B)
+        if rc != 0:
+            pytest.skip("engine 7 does not plan %s at B=%d: %s" % (name, B, msg))
     return request.param
 
 
@@ -37,8 +47,8 @@ def gpu_T(name):
 
 
 def cuda_model(sc, engine):
-    """The case's module on the device.  Both engines plan every case at the batches used here
-    (tests/test_shape_coverage_host.py checks the plans without a GPU)."""
+    """The case's module on the device, planned by the engine the test asks for (the `engine` fixture skips a case
+    engine 7 does not plan; tests/test_shape_coverage_host.py checks the plans without a GPU)."""
     m = fresh_module(sc.kw, sc.sd).cuda()
     assert m._get_engine().plan(sc.B)["engine"] == engine
     return m

@@ -56,7 +56,21 @@ EXPECT = {
     "wide_rs": {1: dict(num_ctas=128)},
     "mol_k34": {1: dict(num_ctas=32)},
     "softmax_wide": {1: dict(num_ctas=64), 4: dict(num_ctas=64)},
+    "gauss3_r6": {1: dict(num_ctas=6, rows_x=1, rows_skip=2, rows_head_b=1)},
+    "mol_k1": {1: dict(num_ctas=10, rows_x=1, rows_skip=2, rows_head_b=1)},
+    "mol_k11": {1: dict(num_ctas=26, rows_x=1, rows_skip=1, rows_head_b=2)},
+    "softmax_255": {1: dict(num_ctas=18, rows_x=2, rows_skip=2, rows_head_b=15)},
 }
+RAGGED = ("gauss3_r6", "mol_k1", "mol_k11", "softmax_255")
+# a block count that divides none of the gate half, residual, skip and head (gauss3_r6 has 6 gate pairs, so at most
+# 6 blocks)
+RAGGED_CTAS = {"gauss3_r6": 4, "mol_k1": 4, "mol_k11": 7, "softmax_255": 7}
+
+
+def ragged(n, P):
+    """n rows over P blocks: the planner sizes every block for ceil(n / P) rows (rows_*), and unless P divides n some
+    blocks own fewer (wn_part), so their row quads are partly filled, or none."""
+    return n != P * cdiv(n, P)
 
 
 @pytest.mark.parametrize("name", NAMES)
@@ -90,9 +104,24 @@ def test_plan_reaches_what_the_case_is_for(name, monkeypatch):
             assert rows_d == 6                       # two quads, the second half filled
         elif name == "k8_global":
             assert rows_d == 14 and max_delay(kw) == 3584
-    if name == "softmax_wide":
+        elif name == "gauss3_r6":
+            assert rows_d == 8                       # two full quads
+        elif name == "mol_k11":
+            assert rows_d == 12                      # three full quads
+        elif name == "softmax_255":
+            assert rows_d == 10                      # three quads, the third half filled
+        if name in RAGGED:
+            # some blocks own fewer rows than the plan's per-block share, or none
+            assert any(ragged(n, P) for n in (R, S, O)), (name, P)
+            # residual, gate half and skip of 2 mod 4, and an odd head
+            assert (R % 4, G2 % 4, S % 4, O % 2) == (2, 2, 2, 1), name
+    if name in ("softmax_wide", "softmax_255"):
         rc, msg = plan_status(cfg, 8)
         assert rc == -1 and "too many rows per block for this batch tile" in msg, msg
+    if name == "softmax_255":
+        # 15 head rows per block: 60 (row, utterance) items at a tile of 4, just under the 64 a block finalises
+        rc, p = plan_status(cfg, 4)
+        assert rc == 0 and p["batch_tile"] == 4 and p["rows_head_b"] * 4 == 60, p
     if name == "eg8":
         # at a tile of 4 nothing is resident: every blob goes through the two streamed slots each step
         rc, p = plan_status(cfg, 4)
@@ -109,13 +138,16 @@ def host_case(name):
 
 
 def replay_ctas(name):
-    """Block counts to replay the packed image at: the default, and 5 wherever the planner accepts it."""
+    """Block counts to replay the packed image at: the default; 5 where the default is 32; for the ragged shapes, a
+    count at which every vector is ragged."""
     rc, p = plan_status(cfg_of(name), 1)
     assert rc == 0, p
     out = [p["num_ctas"]]
-    rc5, _ = plan_status(cfg_of(name, num_ctas=5), 1)
-    if rc5 == 0 and out[0] == 32:
-        out.append(5)
+    extra = RAGGED_CTAS.get(name, 5 if out[0] == 32 else None)
+    if extra is not None:
+        rc, msg = plan_status(cfg_of(name, num_ctas=extra), 1)
+        assert rc == 0, (name, extra, msg)
+        out.append(extra)
     return out
 
 
@@ -126,6 +158,11 @@ def test_engine5_packed_image_replays_oracle(name, monkeypatch):
     Ps = replay_ctas(name)
     if EXPECT[name][1]["num_ctas"] == 32:
         assert 5 in Ps
+    if name in RAGGED:
+        kw = full_kw(name)
+        P = RAGGED_CTAS[name]
+        assert P in Ps and all(ragged(kw[k] // (2 if k == "gate_channels" else 1), P) for k in (
+            "gate_channels", "residual_channels", "skip_out_channels", "out_channels")), (name, P)
     for P in Ps:
         got = hp5.PackedModel(sc, P).run_teacher_forced(0)
         err = float(np.abs(got - sc.arr["params_tf"][0]).max())

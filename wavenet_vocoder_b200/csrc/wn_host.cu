@@ -1729,6 +1729,7 @@ int32_t wn_stream_close(void* stream) {
 int32_t wn_sample_mol(const float* y_bot, int32_t B, int32_t O, int32_t T, const float* u1_tbk, const float* u2_tb,
                       float* out_bt, void* stream) {
     if (!y_bot || !u1_tbk || !u2_tb || !out_bt) return fail(WN_ERR_INVALID, "null argument");
+    if (B < 1 || T < 1 || O < 1) return fail(WN_ERR_INVALID, "wn_sample_mol: B, O and T must be >= 1");
     if (O % 3 != 0) return fail(WN_ERR_INVALID, "out_channels % 3 != 0 (mixture.py:130)");
     const int n = B * T;
     wn::wn_sample_kernel<<<(n + 255) / 256, 256, 0, (cudaStream_t)stream>>>(y_bot, B, O, T, u1_tbk, u2_tb, out_bt, 0);
@@ -1739,6 +1740,7 @@ int32_t wn_sample_mol(const float* y_bot, int32_t B, int32_t O, int32_t T, const
 int32_t wn_sample_gauss(const float* y_bot, int32_t B, int32_t O, int32_t T, const float* u1_tbk, const float* z_tb,
                         float* out_bt, void* stream) {
     if (!y_bot || !z_tb || !out_bt) return fail(WN_ERR_INVALID, "null argument");
+    if (B < 1 || T < 1 || O < 1) return fail(WN_ERR_INVALID, "wn_sample_gauss: B, O and T must be >= 1");
     if (O != 2 && O % 3 != 0) return fail(WN_ERR_INVALID, "out_channels must be 2 or a multiple of 3 (mixture.py:229-234)");
     if (O > 3 && !u1_tbk) return fail(WN_ERR_INVALID, "u1 required for a mixture");
     const int n = B * T;
