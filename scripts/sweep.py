@@ -87,7 +87,7 @@ def main():
         out = r.stdout.strip().splitlines()
         print("%-60s %s" % (spec, out[-1] if out and r.returncode == 0 else "FAILED rc=%d %s" % (r.returncode, r.stderr[-300:])))
         for ln in r.stderr.splitlines():
-            if ln.startswith("WN_PROF"):
+            if ln.startswith("WN_PROF") and not ln.startswith("WN_PROF_BLOCK"):   # scripts/stage_prof.py reads those
                 print("    " + ln)
         sys.stdout.flush()
 

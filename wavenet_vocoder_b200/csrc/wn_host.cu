@@ -622,7 +622,11 @@ static int32_t launch_chunk(WnHandle* h, const wn_generate_args* a, int b0, int 
     pp.gate_cycles = env_int("WN_GATE_CYCLES", 0);
     pp.prof = nullptr;
     if (env_int("WN_PROF", 0)) {
-        const size_t pb = (size_t)pl.P * 16 * sizeof(long long);
+#ifndef WN_STAGE_PROF
+        return fail(WN_ERR_INVALID, "WN_PROF: this libwn.so has no stage counters; scripts/stage_prof.py builds one with "
+                                    "-DWN_STAGE_PROF");
+#endif
+        const size_t pb = (size_t)pl.P * WN_PROF_SLOTS * sizeof(long long);
         rc = ensure(&h->d_prof, &h->prof_bytes, pb);
         if (rc) return rc;
         CUDA_TRY(cudaMemsetAsync(h->d_prof, 0, pb, st));
@@ -1303,20 +1307,24 @@ int32_t wn_sync(void* handle) {
     if (h->d_prof && env_int("WN_PROF", 0)) {
         std::vector<long long> pc(h->prof_bytes / sizeof(long long));
         CUDA_TRY(cudaMemcpy(pc.data(), h->d_prof, h->prof_bytes, cudaMemcpyDeviceToHost));
-        const char* names5[16] = {"C.poll", "C.gemv", "C.barrier", "C.finalize+publish", "C.acquire+pre", "C.head",
-                                  "C.sample+sync", "C.x0", "D.wait_stash", "D.gemv", "D.finalize", "D.sample+sync",
-                                  "-", "-", "-", "-"};
-        const char* names7[16] = {"-", "-", "-", "-", "-", "-", "-", "-",
-                                  "W0.acquire_blob+pre", "W0.wait_input", "W0.critical_passes", "W0.deferred+release",
-                                  "-", "-", "-", "-"};
-        const char** names = h->engine == 7 ? names7 : names5;
-        const int P = (int)(pc.size() / 16);
-        for (int i = 0; i < 12; ++i) {
-            long long mn = pc[i], mx = pc[i], sum = 0;
-            for (int p = 0; p < P; ++p) { mn = std::min(mn, pc[p * 16 + i]); mx = std::max(mx, pc[p * 16 + i]); sum += pc[p * 16 + i]; }
-            fprintf(stderr, "WN_PROF %-20s mean %12.0f  min %12lld  max %12lld cycles\n", names[i], (double)sum / P, mn, mx);
+        if (h->engine != 7) {
+            // the per-block stage profile (wn_kernel.cuh, WN_PROF_SLOTS), one line per block for scripts/stage_prof.py
+            const int P = (int)(pc.size() / WN_PROF_SLOTS);
+            for (int p = 0; p < P; ++p) {
+                fprintf(stderr, "WN_PROF_BLOCK %d", p);
+                for (int i = 0; i < WN_PROF_SLOTS; ++i) fprintf(stderr, " %lld", pc[(size_t)p * WN_PROF_SLOTS + i]);
+                fprintf(stderr, "\n");
+            }
+            fprintf(stderr, "WN_PROF L2 prefetch distance %d blobs\n", h->last_l2_pf);
+        } else {
+            const char* names7[4] = {"W0.acquire_blob+pre", "W0.wait_input", "W0.critical_passes", "W0.deferred+release"};
+            const int P = (int)(pc.size() / 16);
+            for (int i = 8; i < 12; ++i) {
+                long long mn = pc[i], mx = pc[i], sum = 0;
+                for (int p = 0; p < P; ++p) { mn = std::min(mn, pc[p * 16 + i]); mx = std::max(mx, pc[p * 16 + i]); sum += pc[p * 16 + i]; }
+                fprintf(stderr, "WN_PROF %-20s mean %12.0f  min %12lld  max %12lld cycles\n", names7[i - 8], (double)sum / P, mn, mx);
+            }
         }
-        if (h->engine != 7) fprintf(stderr, "WN_PROF L2 prefetch distance %d blobs\n", h->last_l2_pf);
     }
     if (err[0] != 0) {
         cudaMemset(h->d_err, 0, sizeof(err));

@@ -83,7 +83,7 @@ struct WnPtrs {
     int noise_kind;
     unsigned long long seed;
     long long timeout_cycles;
-    long long* prof;           // optional [P][8] cycle counters (scripts/sweep.py --prof)
+    long long* prof;           // [P][WN_PROF_SLOTS] stage profile (-DWN_STAGE_PROF builds only, scripts/stage_prof.py)
     int warp_reverse;          // 1: logical warp = 9 - physical warp (the issue arbiter favours high warp ids)
     int gate_cycles;           // the critical group does not poll an exchange earlier than this after its own publish
     // ---- streaming (wn_stream_generate): a launch continues an utterance at absolute step t_base
@@ -291,19 +291,18 @@ __device__ __forceinline__ float u01(uint32_t r) {   // (0,1), then mapped like 
 }
 
 
-// slow path of every spin loop: has another block faulted / have we waited too long?
-__device__ __noinline__ bool wn_check_abort(volatile int* s_abort, int* err, long long timeout, uint32_t what, int p,
-                                            long long& t0) {
-    if (*s_abort) return true;
+// slow path of every spin loop: has another block faulted / have we waited too long?  `t0` is the clock of the
+// wait's first check (0 before it); returns the value to pass next time, or -1 to abort.  Passed by value: a
+// reference would put it on the stack, and every wait of the stage loop would begin with a local-memory store.
+__device__ __noinline__ long long wn_check_abort(volatile int* s_abort, int* err, long long timeout, uint32_t what,
+                                                 int p, long long t0) {
+    if (*s_abort) return -1;
     if (ld_flag(err) != 0) {
         *s_abort = 1;
-        return true;
+        return -1;
     }
     const long long now = clock64();
-    if (t0 == 0) {
-        t0 = now;
-        return false;
-    }
+    if (t0 == 0) return now;
     if (now - t0 > timeout) {
         if (atomicCAS(err, 0, 1) == 0) {
             err[1] = (int)what;
@@ -311,10 +310,37 @@ __device__ __noinline__ bool wn_check_abort(volatile int* s_abort, int* err, lon
             err[3] = (int)threadIdx.x;
         }
         *s_abort = 1;
-        return true;
+        return -1;
     }
-    return false;
+    return t0;
 }
+
+// Stage profile (scripts/stage_prof.py): cycle counters per block, compiled only with -DWN_STAGE_PROF so that the
+// shipped kernels keep no counter state across the step loop.  Lane 0 of each warp adds its own phases:
+//   critical warp w   [w*12, w*12+12)  stages 1..L-1: acquire+pre, poll, stash, weight load+FMA, shuffle reduce,
+//                                      quad_store, barrier (arrival -> release), finalize, publish, wait for the
+//                                      deferred group; then stages 0, L and the head; then the step tail
+//   critical skew     48: sum over stages 1..L-1 of (last - first arrival at the group barrier), 49: stages counted,
+//                     50+w: stages at which warp w arrived last
+//   deferred warp w   [56+w*6, 56+w*6+6): wait for the stash, unstash, weight load+FMA+reduce+store, barrier,
+//                                      finalize (ring / skip writes), the rest of the step
+//   80, 81: TMA warp cycles spent waiting for a free ring slot, and in total; 82, 83: the same for the
+//   conditioning warp
+#define WN_PROF_SLOTS 96
+enum { WN_PC_ACQ, WN_PC_POLL, WN_PC_STASH, WN_PC_FMA, WN_PC_REDUCE, WN_PC_STORE, WN_PC_BAR, WN_PC_FIN, WN_PC_PUB,
+       WN_PC_DDONE, WN_PC_HEAD, WN_PC_TAIL, WN_PC_CRIT };
+enum { WN_PD_WAIT, WN_PD_UNSTASH, WN_PD_GEMV, WN_PD_BAR, WN_PD_FIN, WN_PD_REST, WN_PC_DEF };
+#ifdef WN_STAGE_PROF
+#define WN_PROF_DECL(N) const bool prof_ = (pp.prof != nullptr) && lane == 0; long long pc_[N] = {}, tc_ = 0;
+#define WN_PROF_START() if (prof_) tc_ = clock64();
+#define WN_TICK(i) if (prof_) { const long long now_ = clock64(); pc_[i] += now_ - tc_; tc_ = now_; }
+#define WN_PROF_STORE(base, N) if (prof_) { for (int i_ = 0; i_ < (N); ++i_) pp.prof[(size_t)p * WN_PROF_SLOTS + (base) + i_] = pc_[i_]; }
+#else
+#define WN_PROF_DECL(N)
+#define WN_PROF_START()
+#define WN_TICK(i)
+#define WN_PROF_STORE(base, N)
+#endif
 
 // ------------------------------------------------------------------------------------------
 #define WN_NTC 128                 // threads of one compute group (4 warps)
@@ -394,7 +420,8 @@ struct Engine {
 
     // ---- watchdog: a stuck wait sets the device fault word and makes every block unwind
     __device__ __forceinline__ bool check_abort(uint32_t what, long long& t0) {
-        return wn_check_abort(s_abort, pp.err, pp.timeout_cycles, what, p, t0);
+        t0 = wn_check_abort(s_abort, pp.err, pp.timeout_cycles, what, p, t0);
+        return t0 < 0;
     }
     // `relaxed` waits (anything off the critical path) back off with nanosleep so that they do not
     // take issue slots and LSU bandwidth from the critical warp of the same SM sub-partition
@@ -630,10 +657,20 @@ struct Engine {
         }
         const uint64_t pol = l2_policy_evict_first();
         int i = pl.nres;
+#ifdef WN_STAGE_PROF
+        const long long t_begin = clock64();
+        long long t_wait = 0;
+#endif
         for (uint32_t js = 0; js < total; ++js) {
             const uint32_t s = js % (uint32_t)pl.nring, u = js / (uint32_t)pl.nring;
             if (u > 0) {
+#ifdef WN_STAGE_PROF
+                const long long t_w = clock64();
+#endif
                 if (!wait_bar<true>(&bar_empty[s], (u - 1) & 1u, 0x40000000u | s)) return;
+#ifdef WN_STAGE_PROF
+                t_wait += clock64() - t_w;
+#endif
             }
             if (dist > 0 && js + dist < total) {
                 prefetch_l2(base + wn_blob_off(pl, ipf), (uint32_t)wn_blob_floats(pl, ipf) * 4u);
@@ -645,6 +682,12 @@ struct Engine {
             bulk_g2s_hint(slots + (size_t)(pl.nres + s) * pl.slot_floats, base + wn_blob_off(pl, i), bytes, fb, pol);
             if (++i == pl.nblobs) i = pl.nres;
         }
+#ifdef WN_STAGE_PROF
+        if (pp.prof != nullptr) {
+            pp.prof[(size_t)p * WN_PROF_SLOTS + 80] = t_wait;
+            pp.prof[(size_t)p * WN_PROF_SLOTS + 81] = clock64() - t_begin;
+        }
+#endif
     }
 
     // ======================================================================================
@@ -656,10 +699,20 @@ struct Engine {
         constexpr int NV = 4 * BT;
         constexpr int M = ilog2c(NV);
         const float* cw = pp.cwpack + (size_t)p * pl.cta_cw_floats;
+#ifdef WN_STAGE_PROF
+        const long long t_begin = clock64();
+        long long t_wait = 0;
+#endif
         for (int t = 0; t < T; ++t) {
             const int par = t & 1, u = t >> 1;
             if (u > 0) {
+#ifdef WN_STAGE_PROF
+                const long long t_w = clock64();
+#endif
                 if (!wait_bar<true>(&bar_cempty[par], (u - 1) & 1u, 0x20000000u)) return;
+#ifdef WN_STAGE_PROF
+                t_wait += clock64() - t_w;
+#endif
             }
             float ct[BT][WN_MAX_CI];
 #pragma unroll
@@ -700,6 +753,12 @@ struct Engine {
             __syncwarp();
             if (lane == 0) mbar_arrive(&bar_cfull[par]);
         }
+#ifdef WN_STAGE_PROF
+        if (pp.prof != nullptr && lane == 0) {
+            pp.prof[(size_t)p * WN_PROF_SLOTS + 82] = t_wait;
+            pp.prof[(size_t)p * WN_PROF_SLOTS + 83] = clock64() - t_begin;
+        }
+#endif
     }
 
     // ======================================================================================
@@ -977,9 +1036,13 @@ struct Engine {
         if (grpA) it_x = -1;
         const int pa_idx = it_y >= 0 ? (2 * (it_y / BT)) * BT + (it_y % BT) : 0;   // [row a_j][b]; row b_j is BT further
         float xr[ER][BT], yr[EG][BT];
-        const bool prof = (pp.prof != nullptr) && tid == 0;
-        long long pc[8] = {0, 0, 0, 0, 0, 0, 0, 0}, tc = 0;
-#define WN_TICK(i) if (prof) { const long long now_ = clock64(); pc[i] += now_ - tc; tc = now_; }
+        WN_PROF_DECL(WN_PC_CRIT)
+#ifdef WN_STAGE_PROF
+        // arrival at the group barrier (low 32 bits of the clock), by stage parity: the last 4 of the 2*nblobs+8
+        // mbarrier words, which no mbarrier uses (no static shared memory: it would shrink the dynamic map)
+        volatile uint32_t* s_arrive = reinterpret_cast<volatile uint32_t*>(bar_full + 2 * pl.nblobs + 4);
+        long long skew = 0, nskew = 0, nlast[WN_GW] = {};
+#endif
         int nstash = 0;      // stashes published so far == deferred stages started
         int ndone = 0;       // deferred stages this group has waited for
         long long t_pub = clock64();
@@ -987,11 +1050,11 @@ struct Engine {
 
         for (int t = 0; t < T; ++t) {
             const uint32_t tagbase = (uint32_t)t * NEID + 1u;
-            if (prof) tc = clock64();
+            WN_PROF_START();
             bool step_dead = false;
             do {
                 make_x0(xr);
-                WN_TICK(7);
+                WN_TICK(WN_PC_TAIL);
                 // ------------------------------------------------------------ stage 0: layer 0 from x_0
                 {
                     const float* W = acquire_blob(t, 0);
@@ -999,9 +1062,7 @@ struct Engine {
                     if (it_y >= 0) { pre_a = pre[pa_idx]; pre_b = pre[pa_idx + BT]; }
                     float* r1 = red1;                                   // partials buffers alternate by stage
                     gemv<ER>(W + pl.fb_Zx, NQ_A, R, xr, r1);
-                    WN_TICK(1);
                     if (bar_or_n<1, WN_NTC>(dead)) { step_dead = true; break; }
-                    WN_TICK(2);
                     if (it_y >= 0) {
                         const int fr = it_y / BT, fb = it_y % BT;
                         const float a = red_sum(r1, 2 * fr, fb) + pre_a;
@@ -1010,14 +1071,14 @@ struct Engine {
                     }
                     release_blob(t, 0);
                     t_pub = clock64();
-                    WN_TICK(3);
+                    WN_TICK(WN_PC_HEAD);
                 }
                 // ------------------------------------------------------------ stages 1..L-1
                 for (int s = 1; s < L; ++s) {
                     const float* W = acquire_blob(t, s);
                     float pre_a = 0.f, pre_b = 0.f;
                     if (it_y >= 0) { pre_a = pre[pa_idx + s * pl.RA4 * BT]; pre_b = pre[pa_idx + s * pl.RA4 * BT + BT]; }
-                    WN_TICK(4);
+                    WN_TICK(WN_PC_ACQ);
                     {
                         const int e0 = pl.ex_yx + (s - 1) * YX;
                         const uint32_t tag = tagbase + wn_eid_yx(s - 1);
@@ -1025,11 +1086,12 @@ struct Engine {
                         if (s >= 2) poll_vec2<EG, ER>(xin, e0, G2, yr, e0 + G2, R, xr, tag);
                         else poll_vec<EG>(xin, e0, G2, tag, yr);      // x_0 is already in registers
                     }
-                    WN_TICK(0);
+                    WN_TICK(WN_PC_POLL);
                     float* xst = xs + (size_t)(s & 1) * R * BT;
                     float* r1 = red1 + (size_t)(s & 1) * pl.red1_floats;
                     stash<ER>(xst, R, xr);
                     stash<EG>(ys + (size_t)(s & 1) * G2 * BT, G2, yr);
+                    WN_TICK(WN_PC_STASH);
                     // gate pre-activations of layer s (quads [0,NQ_A)) and residual rows x_s (quads [NQ_A,nqc))
                     for (int q = 0; q < nqc; q += NA) {
                         float acc[NA][NV];
@@ -1045,37 +1107,64 @@ struct Engine {
                                 quad_fma<EG>(W + pl.lb_Xo + (size_t)(qq - NQ_A) * G2 * 4, G2, yr, acc[h]);
                             }
                         }
+                        WN_TICK(WN_PC_FMA);
                         reduce_scatter_multi<NA, NV>(acc, lane);
+                        WN_TICK(WN_PC_REDUCE);
 #pragma unroll
                         for (int h = 0; h < NA; ++h)
                             if (q + h < nqc) quad_store(acc[h], q + h, r1);
+                        WN_TICK(WN_PC_STORE);
                     }
-                    WN_TICK(1);
+#ifdef WN_STAGE_PROF
+                    if (prof_) s_arrive[(s & 1) * WN_GW + gw] = (uint32_t)tc_;
+#endif
                     if (bar_or_n<1, WN_NTC>(dead)) { step_dead = true; break; }
-                    if (gt == 0) {          // stash complete (the barrier ordered every thread's writes)
+                    WN_TICK(WN_PC_BAR);
+#ifdef WN_STAGE_PROF
+                    if (prof_ && gw == 0) {
+                        const uint32_t a0 = s_arrive[(s & 1) * WN_GW];
+                        int lo = 0, hi = 0, last = 0;
+                        for (int w = 1; w < WN_GW; ++w) {
+                            const int a = (int)(s_arrive[(s & 1) * WN_GW + w] - a0);
+                            lo = min(lo, a);
+                            if (a > hi) { hi = a; last = w; }
+                        }
+                        skew += hi - lo;
+                        ++nskew;
+                        ++nlast[last];
+                    }
+#endif
+                    // stash complete (the barrier ordered every thread's writes).  The last thread of the group hands
+                    // it over: it publishes nothing unless a block owns 64 rows of a vector, whereas thread 0 publishes
+                    // a gate output, and the fence would delay that publish in every stage.
+                    if (gt == WN_NTC - 1) {
                         __threadfence_block();
                         *s_stash_cnt = nstash + 1;
                     }
                     ++nstash;
-                    WN_TICK(2);
                     const uint32_t tag = tagbase + wn_eid_yx(s);
+                    float vy = 0.f, vx = 0.f;
                     if (it_y >= 0) {
                         const int fr = it_y / BT, fb = it_y % BT;
                         const float a = red_sum(r1, 2 * fr, fb) + pre_a;
                         const float g = red_sum(r1, 2 * fr + 1, fb) + pre_b;
-                        publish(pl.ex_yx + s * YX + y0 + fr, fb, cp_y, gate(a, g), tag);
+                        vy = gate(a, g);
                     }
                     if (it_x >= 0) {
                         // modules.py:160-162  x_s = (conv1x1_out(y_{s-1}) + x_{s-1}) * sqrt(0.5)
                         const int fr = it_x / BT, fb = it_x % BT;
                         const float o = red_sum(r1, NQ_A * 4 + fr, fb) + W[pl.lb_xb + fr];
-                        publish(pl.ex_yx + s * YX + G2 + x0r + fr, fb, cp_x, (o + xst[(x0r + fr) * BT + fb]) * RSQRT2, tag);
+                        vx = (o + xst[(x0r + fr) * BT + fb]) * RSQRT2;
                     }
+                    WN_TICK(WN_PC_FIN);
+                    if (it_y >= 0) publish(pl.ex_yx + s * YX + y0 + it_y / BT, it_y % BT, cp_y, vy, tag);
+                    if (it_x >= 0) publish(pl.ex_yx + s * YX + G2 + x0r + it_x / BT, it_x % BT, cp_x, vx, tag);
                     release_blob(t, s);
                     t_pub = clock64();
+                    WN_TICK(WN_PC_PUB);
                     // the stash of stage s+1 reuses the buffer of stage s-1: the deferred group must be done with it
                     if (s >= 2) { wait_count(s_ddone_cnt, WN_GW * (ndone + 1), 0x08000000u); ++ndone; }
-                    WN_TICK(3);
+                    WN_TICK(WN_PC_DDONE);
                 }
                 if (step_dead) break;
                 // ------------------------------------------------------------ stage L: skip of the last layer
@@ -1086,20 +1175,17 @@ struct Engine {
                     if (L >= 2) poll_vec2<EG, ER>(xin, e0, G2, yr, e0 + G2, R, xr, tag);
                     else poll_vec<EG>(xin, e0, G2, tag, yr);
                 }
-                WN_TICK(0);
                 stash<ER>(xs + (size_t)(L & 1) * R * BT, R, xr);
                 float* r1 = red1 + (size_t)(L & 1) * pl.red1_floats;
                 gemv<EG>(H + pl.tb_Sk, pl.NQ_BS, G2, yr, r1);
-                WN_TICK(1);
                 if (bar_or_n<1, WN_NTC>(dead)) { step_dead = true; break; }
-                if (gt == 0) {
+                if (gt == WN_NTC - 1) {     // not a publisher of the skip rows (see the layer stages)
                     __threadfence_block();
                     *s_stash_cnt = nstash + 1;
                 }
                 ++nstash;
                 // skip rows of layers 0..L-2 were accumulated by the deferred group: wait for its stage L-1
                 if (L >= 2) { wait_count(s_ddone_cnt, WN_GW * (ndone + 1), 0x08000001u); ++ndone; }
-                WN_TICK(2);
                 if (it_s >= 0) {
                     // (s_0 + ... + s_{L-2}) + s_{L-1}, * sqrt(1/L), first ReLU of the head (wavenet.py:312-315)
                     const int fr = it_s / BT, fb = it_s % BT;
@@ -1107,7 +1193,6 @@ struct Engine {
                     if (L >= 2) tot = skipacc[it_s] + tot;
                     publish(pl.ex_sk + s0 + fr, fb, cp_s, fmaxf(tot * pl.skip_scale, 0.f), tagbase + wn_eid_sk(pl));
                 }
-                WN_TICK(3);
                 // ---------------------------------------------------------------- head (wavenet.py:315-319)
                 float* r1a = red1 + (size_t)((L + 1) & 1) * pl.red1_floats;
                 if (na > 0) {
@@ -1136,7 +1221,7 @@ struct Engine {
                                         poll_vec<E>(xin, pl.ex_h2, O, tagbase + wn_eid_h2(pl), h);
                                         stash<E>(hs, O, h); });
                 }
-                WN_TICK(5);
+                WN_TICK(WN_PC_HEAD);
             } while (false);
             // ---- both groups meet: sampler (one warp per utterance), then the next step
             if (bar_groups(dead || step_dead)) return;
@@ -1144,12 +1229,17 @@ struct Engine {
             if (L >= 1) ++ndone;
             step_tail(t);
             if (bar_groups(false)) return;
-            WN_TICK(6);
+            WN_TICK(WN_PC_TAIL);
         }
-        if (prof) {
-            for (int i = 0; i < 8; ++i) pp.prof[(size_t)p * 16 + i] = pc[i];
+        WN_PROF_STORE(gw * WN_PC_CRIT, WN_PC_CRIT)
+#ifdef WN_STAGE_PROF
+        if (prof_ && gw == 0) {
+            long long* out = pp.prof + (size_t)p * WN_PROF_SLOTS;
+            out[48] = skew;
+            out[49] = nskew;
+            for (int w = 0; w < WN_GW; ++w) out[50 + w] = nlast[w];
         }
-#undef WN_TICK
+#endif
     }
 
     // head outputs are in hs: optional dump, sampling, feedback for the next step (all 8 compute warps)
@@ -1188,9 +1278,7 @@ struct Engine {
         const int qoff = (kw > 1 ? NQ_D : 0);
         const int nring_items = (kw - 1) * pl.RA * BT, nskip_items = ns * BT;
         float xr[ER][BT], yr[EG][BT];
-        const bool prof = (pp.prof != nullptr) && gt == 0;
-        long long pc[4] = {0, 0, 0, 0}, tc = 0;
-#define WN_TICK(i) if (prof) { const long long now_ = clock64(); pc[i] += now_ - tc; tc = now_; }
+        WN_PROF_DECL(WN_PC_DEF)
         int nstash = 0;
 
         // one deferred stage: `Td` = older taps of `layer` (uses x), `Sk`/`skb` = skip rows of `layer`
@@ -1198,9 +1286,10 @@ struct Engine {
         auto stage = [&](int t, int s, int layer, const float* Td, const float* Sk, const float* skb) {
             wait_count<true>(s_stash_cnt, nstash + 1, 0x04000000u);
             ++nstash;
-            WN_TICK(0);
+            WN_TICK(WN_PD_WAIT);
             unstash<ER>(xs + (size_t)(s & 1) * R * BT, R, xr);
             if (Sk) unstash<EG>(ys + (size_t)(s & 1) * G2 * BT, G2, yr);
+            WN_TICK(WN_PD_UNSTASH);
             float* red = red2 + (size_t)(s & 1) * pl.red2_floats;
             const int nq = Sk ? nqd : qoff;
             for (int q = 0; q < nq; q += NA) {
@@ -1218,8 +1307,9 @@ struct Engine {
                 for (int h = 0; h < NA; ++h)
                     if (q + h < nq) quad_store(acc[h], q + h, red);
             }
-            WN_TICK(1);
+            WN_TICK(WN_PD_GEMV);
             const bool d = bar_or_n<2, WN_NTC>(dead);
+            WN_TICK(WN_PD_BAR);
             if (!d) {
                 // older-tap products of `layer` -> history ring (consumed at steps t+d, t+2d, conv.py:32-44)
                 for (int f = gt; f < nring_items; f += WN_NTC) {
@@ -1239,14 +1329,14 @@ struct Engine {
             __threadfence_block();
             __syncwarp();
             if (lane == 0) atomicAdd((int*)s_ddone_cnt, 1);
-            WN_TICK(2);
+            WN_TICK(WN_PD_FIN);
             return d;
         };
 
         build_pre(0);
         if (bar_groups(dead)) return;
         for (int t = 0; t < T; ++t) {
-            if (prof) tc = clock64();
+            WN_PROF_START();
             bool step_dead = false;
             release_blob(t, 0);                       // stage 0 has no deferred work
             for (int s = 1; s < L && !step_dead; ++s) {
@@ -1267,12 +1357,9 @@ struct Engine {
             if (bar_groups(dead || step_dead)) return;
             step_tail(t);
             if (bar_groups(false)) return;
-            WN_TICK(3);
+            WN_TICK(WN_PD_REST);
         }
-        if (prof) {
-            for (int i = 0; i < 4; ++i) pp.prof[(size_t)p * 16 + 8 + i] = pc[i];
-        }
-#undef WN_TICK
+        WN_PROF_STORE(56 + gw * WN_PC_DEF, WN_PC_DEF)
     }
 };
 
