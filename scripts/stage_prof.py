@@ -27,9 +27,10 @@ from sweep import CFGS  # noqa: E402
 from wavenet_vocoder_b200 import _native  # noqa: E402
 
 SLOTS = 96                      # WN_PROF_SLOTS
-NCRIT, NDEF = 12, 6             # counters per critical / deferred warp (WN_PC_CRIT, WN_PC_DEF)
-CRIT = ["acquire+pre", "poll", "stash", "weight load+FMA", "shuffle reduce", "quad_store", "barrier",
-        "finalize", "publish", "wait for deferred"]
+NCRIT, NDEF = 13, 6             # counters per critical / deferred warp (WN_PC_CRIT, WN_PC_DEF)
+SKEW, DEFB, TMA, COND = 52, 58, 82, 84   # WN_PS_SKEW, WN_PS_DEF, WN_PS_TMA, WN_PS_COND
+CRIT = ["acquire+pre", "poll", "stash", "weight load+FMA issue", "wait for FMA results",
+        "shuffle reduce", "quad_store", "barrier", "finalize", "publish", "wait for deferred"]
 DEF = ["wait for stash", "unstash", "load+FMA+reduce+store", "barrier", "finalize"]
 
 
@@ -76,15 +77,15 @@ def report(pc, timing, cfg, T):
     tot = [pc[:, w * NCRIT:w * NCRIT + len(CRIT)].sum(1) / ncs for w in range(4)]
     out["crit"]["stage total"] = [float(c.mean()) for c in tot]
     print("| stage total | %s |" % " | ".join(cell(c) for c in tot))
-    for i, name in ((10, "stages 0, L + head, per step"), (11, "x_0 + step tail, per step")):
+    for i, name in ((11, "stages 0, L + head, per step"), (12, "x_0 + step tail, per step")):
         cols = [pc[:, w * NCRIT + i] / T for w in range(4)]
         out["crit"][name] = [float(c.mean()) for c in cols]
         print("| %s | %s |" % (name, " | ".join(cell(c) for c in cols)))
     step = pc[:, 0:NCRIT].sum(1) / T
     out["crit"]["warp 0 step"] = float(step.mean())
     print("| warp 0, whole step | %s | | | |" % cell(step))
-    skew = pc[:, 48] / np.maximum(pc[:, 49], 1)
-    last = pc[:, 50:54] / np.maximum(pc[:, 49:50], 1)
+    skew = pc[:, SKEW] / np.maximum(pc[:, SKEW + 1], 1)
+    last = pc[:, SKEW + 2:SKEW + 6] / np.maximum(pc[:, SKEW + 1:SKEW + 2], 1)
     out["skew"] = float(skew.mean())
     out["last_share"] = [float(v) for v in last.mean(0)]
     print("\narrival skew at the critical group's barrier (last - first warp): %s cycles per stage" % cell(skew))
@@ -93,13 +94,13 @@ def report(pc, timing, cfg, T):
     print("| phase | " + " | ".join("warp %d" % (4 + w) for w in range(4)) + " |")
     print("|---|" + "---|" * 4)
     for i, name in enumerate(DEF):
-        cols = [pc[:, 56 + w * NDEF + i] / nds for w in range(4)]
+        cols = [pc[:, DEFB + w * NDEF + i] / nds for w in range(4)]
         out["deferred"][name] = [float(c.mean()) for c in cols]
         print("| %s | %s |" % (name, " | ".join(cell(c) for c in cols)))
-    cols = [pc[:, 56 + w * NDEF + 5] / T for w in range(4)]
+    cols = [pc[:, DEFB + w * NDEF + 5] / T for w in range(4)]
     out["deferred"]["pre-sums + step tail, per step"] = [float(c.mean()) for c in cols]
     print("| pre-sums + step tail, per step | %s |" % " | ".join(cell(c) for c in cols))
-    for base, name in ((80, "TMA warp"), (82, "conditioning warp")):
+    for base, name in ((TMA, "TMA warp"), (COND, "conditioning warp")):
         wait, total = pc[:, base] / T, pc[:, base + 1] / T
         out[name] = {"wait_per_step": float(wait.mean()), "total_per_step": float(total.mean())}
         print("\n%s: waits %s of %s cycles per step" % (name, cell(wait), cell(total)), end="")

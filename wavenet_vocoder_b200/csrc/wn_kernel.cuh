@@ -317,28 +317,35 @@ __device__ __noinline__ long long wn_check_abort(volatile int* s_abort, int* err
 
 // Stage profile (scripts/stage_prof.py): cycle counters per block, compiled only with -DWN_STAGE_PROF so that the
 // shipped kernels keep no counter state across the step loop.  Lane 0 of each warp adds its own phases:
-//   critical warp w   [w*12, w*12+12)  stages 1..L-1: acquire+pre, poll, stash, weight load+FMA, shuffle reduce,
+//   critical warp w   [w*13, w*13+13)  stages 1..L-1: acquire+pre, poll, stash, weight load+FMA issue, wait for the
+//                                      FMA results (and so for the weight reads they consume), shuffle reduce,
 //                                      quad_store, barrier (arrival -> release), finalize, publish, wait for the
 //                                      deferred group; then stages 0, L and the head; then the step tail
-//   critical skew     48: sum over stages 1..L-1 of (last - first arrival at the group barrier), 49: stages counted,
-//                     50+w: stages at which warp w arrived last
-//   deferred warp w   [56+w*6, 56+w*6+6): wait for the stash, unstash, weight load+FMA+reduce+store, barrier,
+//   critical skew     52: sum over stages 1..L-1 of (last - first arrival at the group barrier), 53: stages counted,
+//                     54+w: stages at which warp w arrived last
+//   deferred warp w   [58+w*6, 58+w*6+6): wait for the stash, unstash, weight load+FMA+reduce+store, barrier,
 //                                      finalize (ring / skip writes), the rest of the step
-//   80, 81: TMA warp cycles spent waiting for a free ring slot, and in total; 82, 83: the same for the
+//   82, 83: TMA warp cycles spent waiting for a free ring slot, and in total; 84, 85: the same for the
 //   conditioning warp
 #define WN_PROF_SLOTS 96
-enum { WN_PC_ACQ, WN_PC_POLL, WN_PC_STASH, WN_PC_FMA, WN_PC_REDUCE, WN_PC_STORE, WN_PC_BAR, WN_PC_FIN, WN_PC_PUB,
-       WN_PC_DDONE, WN_PC_HEAD, WN_PC_TAIL, WN_PC_CRIT };
+enum { WN_PC_ACQ, WN_PC_POLL, WN_PC_STASH, WN_PC_FMA, WN_PC_READY, WN_PC_REDUCE, WN_PC_STORE, WN_PC_BAR, WN_PC_FIN,
+       WN_PC_PUB, WN_PC_DDONE, WN_PC_HEAD, WN_PC_TAIL, WN_PC_CRIT };
 enum { WN_PD_WAIT, WN_PD_UNSTASH, WN_PD_GEMV, WN_PD_BAR, WN_PD_FIN, WN_PD_REST, WN_PC_DEF };
+enum { WN_PS_SKEW = 4 * WN_PC_CRIT, WN_PS_DEF = WN_PS_SKEW + 6, WN_PS_TMA = WN_PS_DEF + 4 * WN_PC_DEF,
+       WN_PS_COND = WN_PS_TMA + 2 };
+static_assert(WN_PS_COND + 2 <= WN_PROF_SLOTS, "stage profile slots");
 #ifdef WN_STAGE_PROF
 #define WN_PROF_DECL(N) const bool prof_ = (pp.prof != nullptr) && lane == 0; long long pc_[N] = {}, tc_ = 0;
 #define WN_PROF_START() if (prof_) tc_ = clock64();
 #define WN_TICK(i) if (prof_) { const long long now_ = clock64(); pc_[i] += now_ - tc_; tc_ = now_; }
+// the same after a shared-memory store of `v`: the store, and so the clock read behind it, waits until v is computed
+#define WN_TICK_AFTER(i, sink, v) if (prof_) { *reinterpret_cast<volatile float*>(sink) = (v); } WN_TICK(i)
 #define WN_PROF_STORE(base, N) if (prof_) { for (int i_ = 0; i_ < (N); ++i_) pp.prof[(size_t)p * WN_PROF_SLOTS + (base) + i_] = pc_[i_]; }
 #else
 #define WN_PROF_DECL(N)
 #define WN_PROF_START()
 #define WN_TICK(i)
+#define WN_TICK_AFTER(i, sink, v)
 #define WN_PROF_STORE(base, N)
 #endif
 
@@ -507,13 +514,27 @@ struct Engine {
         }
         return bad;
     }
+    // At a tile of 1 the polls are warp-uniform: every lane repeats its loads until the whole warp's elements have
+    // arrived, and the watchdog's verdict is shared.  A lane that left the loop on its own would run the GEMV in a
+    // divergent branch while other lanes of its warp still poll, and the warp's shuffle reduction would wait for the
+    // last of them (every critical-group thread calls every poll, so all 32 lanes are here).  Larger tiles keep
+    // per-lane polls: with the votes, -Xptxas -v shows more spill in <4,2,2>, <4,4,2,true> and <8,2,2>.
+    static constexpr bool WARP_POLL = BT == 1;
+    __device__ __forceinline__ static bool poll_all(bool mine) {
+        if constexpr (WARP_POLL) return __all_sync(0xffffffffu, mine);
+        else return mine;
+    }
+    __device__ __forceinline__ static bool poll_any(bool mine) {
+        if constexpr (WARP_POLL) return __any_sync(0xffffffffu, mine);
+        else return mine;
+    }
     template <int E>
     __device__ __forceinline__ void poll_vec(const uint2* __restrict__ src, int e0, int K, uint32_t tag,
                                              float (&x)[E][BT]) {
         uint32_t spins = 0;
         long long t0 = 0;
-        while (load_vec<E>(src, e0, K, tag, x) != 0) {
-            if (((++spins) & 63u) == 0 && check_abort(tag, t0)) {
+        while (!poll_all(load_vec<E>(src, e0, K, tag, x) == 0)) {
+            if (((++spins) & 63u) == 0 && poll_any(check_abort(tag, t0))) {
                 dead = true;
                 return;
             }
@@ -527,8 +548,8 @@ struct Engine {
         long long t0 = 0;
         while (true) {
             const uint32_t bad = load_vec<EA>(src, ea, KA, tag, a) | load_vec<EB>(src, eb, KB, tag, b);
-            if (bad == 0) return;
-            if (((++spins) & 63u) == 0 && check_abort(tag, t0)) {
+            if (poll_all(bad == 0)) return;
+            if (((++spins) & 63u) == 0 && poll_any(check_abort(tag, t0))) {
                 dead = true;
                 return;
             }
@@ -556,21 +577,74 @@ struct Engine {
     }
 
     // ---- one row quad (4 rows x K) times the thread's slice of the input vector, accumulated
+    __device__ __forceinline__ static void fma_k(float4 w4, const float (&xk)[BT], float (&acc)[NV]) {
+#pragma unroll
+        for (int b = 0; b < BT; ++b) {
+            acc[0 * BT + b] = fmaf(w4.x, xk[b], acc[0 * BT + b]);
+            acc[1 * BT + b] = fmaf(w4.y, xk[b], acc[1 * BT + b]);
+            acc[2 * BT + b] = fmaf(w4.z, xk[b], acc[2 * BT + b]);
+            acc[3 * BT + b] = fmaf(w4.w, xk[b], acc[3 * BT + b]);
+        }
+    }
     template <int E>
     __device__ __forceinline__ void quad_fma(const float* __restrict__ wq /* [K][4] */, int K,
                                              const float (&x)[E][BT], float (&acc)[NV]) {
 #pragma unroll
         for (int j = 0; j < E; ++j) {
             const int k = elem<E>(j);
-            if (k < K) {
-                const float4 w4 = *reinterpret_cast<const float4*>(wq + (size_t)k * 4);
+            if (k < K) fma_k(*reinterpret_cast<const float4*>(wq + (size_t)k * 4), x[j], acc);
+        }
+    }
+
+    // ---- layer stages 1..L-1: the weights of the first pass of NA quads are read into registers before the poll
+    // (the ring slot is full once acquire_blob returns), so that after the exchange arrives only FMAs are left.
+    // Weight w of that pass, w = h*(EG+ER) + j, is the float4 that multiplies y element j (j < EG; gate quads: M_{s-1},
+    // residual quads: conv1x1_out_{s-1}) or x element j-EG (gate quads only: V_s) in quad h.  The first NPRE of them
+    // are preloaded; the others are read from shared memory when they are used.  The kernel is held to 168 registers
+    // (320 threads, one block per SM): -Xptxas -v shows no more stack or spill than without the preload only for a
+    // tile of 1 with EG + ER <= 6 outside the stream kernels (config 2 is <1,4,2,false>); the other instantiations
+    // read the weights as they multiply.
+    static constexpr int NW0 = NA * (EG + ER);
+    static constexpr int NPRE = (BT == 1 && !STREAM && EG + ER <= 6) ? (NW0 < 8 ? NW0 : 8) : 0;
+    static constexpr int NPRE_A = NPRE > 0 ? NPRE : 1;
+    __device__ __forceinline__ const float* w0y(const float* W, int h, int NQ_A) const {
+        return h < NQ_A ? W + pl.lb_Zy + (size_t)h * pl.G2 * 4 : W + pl.lb_Xo + (size_t)(h - NQ_A) * pl.G2 * 4;
+    }
+    __device__ __forceinline__ void preload0(const float* W, int NQ_A, int nqc, float4 (&wp)[NPRE_A]) {
 #pragma unroll
-                for (int b = 0; b < BT; ++b) {
-                    acc[0 * BT + b] = fmaf(w4.x, x[j][b], acc[0 * BT + b]);
-                    acc[1 * BT + b] = fmaf(w4.y, x[j][b], acc[1 * BT + b]);
-                    acc[2 * BT + b] = fmaf(w4.z, x[j][b], acc[2 * BT + b]);
-                    acc[3 * BT + b] = fmaf(w4.w, x[j][b], acc[3 * BT + b]);
-                }
+        for (int w = 0; w < NPRE; ++w) {
+            const int h = w / (EG + ER), j = w % (EG + ER);
+            const float* src = nullptr;
+            if (j < EG) {
+                const int k = elem<EG>(j);
+                if (h < nqc && k < pl.G2) src = w0y(W, h, NQ_A) + (size_t)k * 4;
+            } else {
+                const int k = elem<ER>(j - EG);
+                if (h < NQ_A && k < pl.R) src = W + pl.lb_Zx + ((size_t)h * pl.R + k) * 4;
+            }
+            wp[w] = src ? *reinterpret_cast<const float4*>(src) : make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+    }
+    // the first pass: quad h sums y[0..EG) then x[0..ER), the order quad_fma sums in
+    __device__ __forceinline__ void pass0(const float* W, int NQ_A, int nqc, const float4 (&wp)[NPRE_A],
+                                          const float (&yr)[EG][BT], const float (&xr)[ER][BT], float (&acc)[NA][NV]) {
+#pragma unroll
+        for (int h = 0; h < NA; ++h) {
+#pragma unroll
+            for (int v = 0; v < NV; ++v) acc[h][v] = 0.f;
+#pragma unroll
+            for (int j = 0; j < EG; ++j) {
+                const int k = elem<EG>(j), w = h * (EG + ER) + j;
+                if (h < nqc && k < pl.G2)
+                    fma_k(w < NPRE ? wp[w] : *reinterpret_cast<const float4*>(w0y(W, h, NQ_A) + (size_t)k * 4), yr[j],
+                          acc[h]);
+            }
+#pragma unroll
+            for (int j = 0; j < ER; ++j) {
+                const int k = elem<ER>(j), w = h * (EG + ER) + EG + j;
+                if (h < NQ_A && k < pl.R)
+                    fma_k(w < NPRE ? wp[w] : *reinterpret_cast<const float4*>(W + pl.lb_Zx + ((size_t)h * pl.R + k) * 4),
+                          xr[j], acc[h]);
             }
         }
     }
@@ -684,8 +758,8 @@ struct Engine {
         }
 #ifdef WN_STAGE_PROF
         if (pp.prof != nullptr) {
-            pp.prof[(size_t)p * WN_PROF_SLOTS + 80] = t_wait;
-            pp.prof[(size_t)p * WN_PROF_SLOTS + 81] = clock64() - t_begin;
+            pp.prof[(size_t)p * WN_PROF_SLOTS + WN_PS_TMA] = t_wait;
+            pp.prof[(size_t)p * WN_PROF_SLOTS + WN_PS_TMA + 1] = clock64() - t_begin;
         }
 #endif
     }
@@ -755,8 +829,8 @@ struct Engine {
         }
 #ifdef WN_STAGE_PROF
         if (pp.prof != nullptr && lane == 0) {
-            pp.prof[(size_t)p * WN_PROF_SLOTS + 82] = t_wait;
-            pp.prof[(size_t)p * WN_PROF_SLOTS + 83] = clock64() - t_begin;
+            pp.prof[(size_t)p * WN_PROF_SLOTS + WN_PS_COND] = t_wait;
+            pp.prof[(size_t)p * WN_PROF_SLOTS + WN_PS_COND + 1] = clock64() - t_begin;
         }
 #endif
     }
@@ -1078,6 +1152,8 @@ struct Engine {
                     const float* W = acquire_blob(t, s);
                     float pre_a = 0.f, pre_b = 0.f;
                     if (it_y >= 0) { pre_a = pre[pa_idx + s * pl.RA4 * BT]; pre_b = pre[pa_idx + s * pl.RA4 * BT + BT]; }
+                    float4 wp[NPRE_A];
+                    if constexpr (NPRE > 0) preload0(W, NQ_A, nqc, wp);
                     WN_TICK(WN_PC_ACQ);
                     {
                         const int e0 = pl.ex_yx + (s - 1) * YX;
@@ -1095,19 +1171,24 @@ struct Engine {
                     // gate pre-activations of layer s (quads [0,NQ_A)) and residual rows x_s (quads [NQ_A,nqc))
                     for (int q = 0; q < nqc; q += NA) {
                         float acc[NA][NV];
+                        if (NPRE > 0 && q == 0) {
+                            pass0(W, NQ_A, nqc, wp, yr, xr, acc);
+                        } else {
 #pragma unroll
-                        for (int h = 0; h < NA; ++h) {
+                            for (int h = 0; h < NA; ++h) {
 #pragma unroll
-                            for (int v = 0; v < NV; ++v) acc[h][v] = 0.f;
-                            const int qq = q + h;
-                            if (qq < NQ_A) {
-                                quad_fma<EG>(W + pl.lb_Zy + (size_t)qq * G2 * 4, G2, yr, acc[h]);
-                                quad_fma<ER>(W + pl.lb_Zx + (size_t)qq * R * 4, R, xr, acc[h]);
-                            } else if (qq < nqc) {
-                                quad_fma<EG>(W + pl.lb_Xo + (size_t)(qq - NQ_A) * G2 * 4, G2, yr, acc[h]);
+                                for (int v = 0; v < NV; ++v) acc[h][v] = 0.f;
+                                const int qq = q + h;
+                                if (qq < NQ_A) {
+                                    quad_fma<EG>(W + pl.lb_Zy + (size_t)qq * G2 * 4, G2, yr, acc[h]);
+                                    quad_fma<ER>(W + pl.lb_Zx + (size_t)qq * R * 4, R, xr, acc[h]);
+                                } else if (qq < nqc) {
+                                    quad_fma<EG>(W + pl.lb_Xo + (size_t)(qq - NQ_A) * G2 * 4, G2, yr, acc[h]);
+                                }
                             }
                         }
                         WN_TICK(WN_PC_FMA);
+                        WN_TICK_AFTER(WN_PC_READY, r1 + (size_t)q * NV * WN_GW + gw, acc[NA - 1][NV - 1]);
                         reduce_scatter_multi<NA, NV>(acc, lane);
                         WN_TICK(WN_PC_REDUCE);
 #pragma unroll
@@ -1235,9 +1316,9 @@ struct Engine {
 #ifdef WN_STAGE_PROF
         if (prof_ && gw == 0) {
             long long* out = pp.prof + (size_t)p * WN_PROF_SLOTS;
-            out[48] = skew;
-            out[49] = nskew;
-            for (int w = 0; w < WN_GW; ++w) out[50 + w] = nlast[w];
+            out[WN_PS_SKEW] = skew;
+            out[WN_PS_SKEW + 1] = nskew;
+            for (int w = 0; w < WN_GW; ++w) out[WN_PS_SKEW + 2 + w] = nlast[w];
         }
 #endif
     }
@@ -1359,7 +1440,7 @@ struct Engine {
             if (bar_groups(false)) return;
             WN_TICK(WN_PD_REST);
         }
-        WN_PROF_STORE(56 + gw * WN_PC_DEF, WN_PC_DEF)
+        WN_PROF_STORE(WN_PS_DEF + gw * WN_PC_DEF, WN_PC_DEF)
     }
 };
 
