@@ -27,7 +27,8 @@ extern "C" {
 #endif
 
 /* 3 = 2 plus streaming (wn_stream_*, wn_upsample_cone, wn_decode_stream); no struct of version 2 changed, and
- * wn_create accepts a wn_config that says 2 */
+ * wn_create accepts a wn_config that says 2.  Fields added later in ABI 3 take a slot of a `reserved` array (zero =
+ * the behaviour before them), so no struct size changed: wn_config.engine, wn_stream_open_args.engine. */
 #define WN_ABI_VERSION 3
 
 typedef enum wn_status {
@@ -73,7 +74,11 @@ typedef struct wn_config {
     int32_t ring_slots;           /* 0 = choose; streaming weight slots in shared memory  */
     int32_t poll_warps;           /* 0 = choose; warps that poll the exchange into shared memory (2..8, larger
                                      values plan as 8); -1 = none, the compute warps poll (engine 7) */
-    int32_t reserved[7];
+    int32_t engine;               /* kernel organisation: 0 = environment variable WN_ENGINE (7, else 5); 5 or 7 = that
+                                     one, whatever WN_ENGINE says; other values are refused (WN_ERR_INVALID).
+                                     wn_create, wn_plan_only and wn_pack_cta follow it (wn_get_plan reports the
+                                     handle's); wn_plan_passes checks it (its table is engine 7's in any case) */
+    int32_t reserved[6];
 } wn_config;
 
 /* One residual layer, HOST pointers, fp32, weight-norm already folded (modules.py:13-18).
@@ -207,12 +212,14 @@ int32_t wn_generate_host(void* handle, const wn_generate_args* args);
 int32_t wn_get_plan(void* handle, int32_t batch, wn_plan_info* out);
 
 /* ---- Streaming (ABI 3): one utterance made in consecutive chunks, bit-identical to one wn_generate call over the
- * whole utterance with the same weights, noise and conditioning, for any split.  What links step t to step t+1 --
- * the older-tap history rings, the fed-back sample, the Philox step -- stays in a device buffer the stream owns.
- * Engine 5 only, at most one batch tile (4 utterances), no teacher forcing.  Several streams may be open on one
- * handle and called in turn; the handle still runs one call at a time, and wn_sync(handle) waits for a chunk. */
+ * whole utterance on the same handle with the same weights, noise and conditioning, for any split.  What links step
+ * t to step t+1 -- the older-tap history rings, the fed-back sample, the Philox step -- stays in a device buffer the
+ * stream owns.  One batch tile per stream: engine 5 (the default) holds 1..4 utterances, engine 7
+ * (wn_stream_open_args.engine = 7, on a handle created with wn_config.engine = 7 and compute warps that poll) 1..8.
+ * No teacher forcing.  Several streams may be open on one handle and called in turn; the handle still runs one call
+ * at a time, and wn_sync(handle) waits for a chunk. */
 typedef struct wn_stream_open_args {
-    int32_t B;                     /* utterances, 1..4                                                             */
+    int32_t B;                     /* utterances, 1..4 (engine 5) or 1..8 (engine 7)                               */
     const float* g;                /* DEVICE (B,gin) or NULL; read once, at open                                    */
     const float* initial;          /* DEVICE, as wn_generate_args; copied at open                                   */
     int32_t initial_index;
@@ -224,7 +231,9 @@ typedef struct wn_stream_open_args {
     uint64_t seed;
     int32_t philox_row0;
     void* stream;                  /* cudaStream_t of the open (it returns after the set-up is complete)            */
-    int32_t reserved[6];
+    int32_t engine;                /* 0 or 5: an engine-5 stream, on an engine-5 handle; 7: an engine-7 stream, on
+                                      an engine-7 handle whose compute warps poll; other values WN_ERR_INVALID    */
+    int32_t reserved[5];
 } wn_stream_open_args;
 
 /* Where a chunk's conditioning FRAMES (wn_generate_args.c_frames, n_frames of them) sit in the utterance. */

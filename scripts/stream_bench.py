@@ -6,7 +6,12 @@ first chunk and the cost of one chunk boundary ((chunked - one chunk) / boundari
 instantiation, so its per-step cost is the one-chunk mode against the one-shot call), medians of --runs runs, and the
 card's name and power limit (nvidia-smi, read only).
 
-    python scripts/stream_bench.py [--T 22050] [--runs 3] [--chunks 256,1024,4096]
+--B 8 --engine 7 makes 8 utterances at once: one engine-7 wn_generate, and one engine-7 stream of 8 (on an engine-7
+handle of the same weights).  --engine 5 with B > 4 runs the one-shot call as wn_generate's consecutive tiles of 4 and
+the stream as streams of at most 4 called in turn, each chunk synchronised; the time to the first chunk is then the
+time until every utterance has its first chunk.  --engine 5,7 alternates the two engines run by run in one process.
+
+    python scripts/stream_bench.py [--T 22050] [--runs 3] [--chunks 256,1024,4096] [--B 1] [--engine 5]
 """
 import argparse
 import json
@@ -41,7 +46,12 @@ def main():
     ap.add_argument("--T", type=int, default=22050)
     ap.add_argument("--runs", type=int, default=3)
     ap.add_argument("--chunks", default="256,1024,4096")
+    ap.add_argument("--B", type=int, default=1, help="utterances")
+    ap.add_argument("--engine", default="5", help="5, 7 or 5,7 (alternated run by run)")
     args = ap.parse_args()
+    engines = [int(e) for e in args.engine.split(",")]
+    assert engines and set(engines) <= {5, 7}, args.engine
+    B = args.B
     from wavenet_vocoder_b200 import WaveNet
     dev = torch.device("cuda", 0)
     torch.manual_seed(0)
@@ -52,53 +62,64 @@ def main():
     eng = m._get_engine()
     T = args.T
     frames = -(-T // 256) + 4
-    mel = torch.randn(1, 80, frames, generator=torch.Generator().manual_seed(1)).to(dev)
-    c = eng.upsample(mel, eng.upsampled_length(frames))[:, :T].contiguous()     # (1,T,80) sample-rate conditioning
+    mel = torch.randn(B, 80, frames, generator=torch.Generator().manual_seed(1)).to(dev)
+    c = eng.upsample(mel, eng.upsampled_length(frames))[:, :T].contiguous()     # (B,T,80) sample-rate conditioning
+    handle = {5: eng, 7: eng.engine7() if 7 in engines else None}
 
-    def one_shot(seed):
+    def one_shot(e, seed):
         t0 = time.perf_counter()
-        y, _ = eng.generate(B=1, T=T, c=c, seed=seed)
+        y, _ = handle[e].generate(B=B, T=T, c=c, seed=seed)
         t1 = time.perf_counter()
         return t1 - t0, t1 - t0, y
 
-    def chunked(n, seed):
-        s = eng.open_stream(B=1, seed=seed)
-        ys, first = [], None
+    def chunked(e, n, seed):
+        tile = B if e == 7 else 4              # engine 5: streams of at most 4 rows, row b draws row b's noise
+        streams = [(handle[e].open_stream(B=min(tile, B - b0), seed=seed, philox_row0=b0, engine=e), b0)
+                   for b0 in range(0, B, tile)]
+        ys, first = [[] for _ in streams], None
         t0 = time.perf_counter()
         for t in range(0, T, n):
             k = min(n, T - t)
-            y, _ = s.generate(k, c=c[:, t:t + k])      # synchronised: the chunk is ready when this returns
-            ys.append(y)
+            for (s, b0), yk in zip(streams, ys):
+                y, _ = s.generate(k, c=c[b0:b0 + s.B, t:t + k])      # synchronised: the chunk is ready when this returns
+                yk.append(y)
             if first is None:
                 first = time.perf_counter() - t0
         total = time.perf_counter() - t0
-        s.close()
-        return total, first, torch.cat(ys, -1)
+        for s, _ in streams:
+            s.close()
+        return total, first, torch.cat([torch.cat(yk, -1) for yk in ys], 0)
 
     modes = [("one_shot", None), ("stream_one_chunk", T)] + [("chunk_%d" % int(n), int(n)) for n in args.chunks.split(",")]
-    res = {}
-    ref = None
+    res = {e: {} for e in engines}
+    ref = {}
     for name, n in modes:
-        fn = one_shot if n is None else (lambda seed, n=n: chunked(n, seed))
-        fn(7)                                           # warm-up
-        tot, fst = [], []
+        tot, fst = {e: [] for e in engines}, {e: [] for e in engines}
+        for e in engines:
+            (one_shot(e, 7) if n is None else chunked(e, n, 7))       # warm-up
         for r in range(args.runs):
-            a, b, y = fn(7)
-            tot.append(a), fst.append(b)
-            if ref is None:
-                ref = y
-            assert torch.equal(y, ref), name + ": chunked output differs from one shot"
-        tot.sort(), fst.sort()
-        res[name] = dict(chunk=n, seconds=tot[len(tot) // 2], samples_per_s=T / tot[len(tot) // 2],
-                         first_chunk_ms=1e3 * fst[len(fst) // 2], runs=tot)
-    one, whole = res["one_shot"]["seconds"], res["stream_one_chunk"]["seconds"]
-    res["stream_one_chunk"]["us_per_step_vs_one_shot"] = 1e6 * (whole - one) / T
-    for name, n in modes[2:]:
-        b = -(-T // n) - 1
-        res[name]["boundaries"] = b
-        res[name]["us_per_boundary"] = 1e6 * (res[name]["seconds"] - whole) / b
-        res[name]["vs_one_shot"] = res[name]["seconds"] / one
-    print(json.dumps(dict(card=card(), T=T, config="cfg2 B=1", modes=res), indent=1))
+            for e in engines:
+                a, b, y = one_shot(e, 7) if n is None else chunked(e, n, 7)
+                tot[e].append(a), fst[e].append(b)
+                if e not in ref:
+                    ref[e] = y
+                assert torch.equal(y, ref[e]), "%s engine %d: chunked output differs from one shot" % (name, e)
+        for e in engines:
+            tot[e].sort(), fst[e].sort()
+            res[e][name] = dict(chunk=n, seconds=tot[e][len(tot[e]) // 2], samples_per_s=B * T / tot[e][len(tot[e]) // 2],
+                                first_chunk_ms=1e3 * fst[e][len(fst[e]) // 2], runs=tot[e])
+    for e in engines:
+        one, whole = res[e]["one_shot"]["seconds"], res[e]["stream_one_chunk"]["seconds"]
+        res[e]["stream_one_chunk"]["us_per_step_vs_one_shot"] = 1e6 * (whole - one) / T
+        for name, n in modes[2:]:
+            b = -(-T // n) - 1
+            res[e][name]["boundaries"] = b
+            res[e][name]["us_per_boundary"] = 1e6 * (res[e][name]["seconds"] - whole) / b
+            res[e][name]["vs_one_shot"] = res[e][name]["seconds"] / one
+    if engines == [5]:
+        print(json.dumps(dict(card=card(), T=T, config="cfg2 B=%d" % B, modes=res[5]), indent=1))
+    else:
+        print(json.dumps(dict(card=card(), T=T, config="cfg2 B=%d" % B, engines=res), indent=1))
 
 
 if __name__ == "__main__":

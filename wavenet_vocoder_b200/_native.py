@@ -15,7 +15,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 LIB_PATH = os.path.join(HERE, "libwn.so")
 SOURCES = [os.path.join(HERE, "csrc", "wn_host.cu")]
-HEADERS = [os.path.join(HERE, "csrc", f) for f in ("wn_plan.h", "wn_kernel.cuh", "wn7_plan.h", "wn7_kernel.cuh",
+HEADERS = [os.path.join(HERE, "csrc", f) for f in ("wn_plan.h", "wn_kernel.cuh", "wn7_plan.h", "wn7_kernel.cuh", "wn7_kernel_body.cuh",
                                                      "wn7_host.cuh", "wn_aux.cuh",
                                                      "wn_dense.cuh")] + [os.path.join(ROOT, "include", "wn.h")]
 
@@ -33,7 +33,7 @@ class wn_config(C.Structure):
     _fields_ = [(n, C.c_int32) for n in (
         "abi_version", "layers", "stacks", "residual_channels", "gate_channels", "skip_channels",
         "out_channels", "kernel_size", "cin_channels", "gin_channels", "input_kind", "head_kind",
-        "device", "num_ctas", "exchange_copies", "ring_slots", "poll_warps")] + [("reserved", C.c_int32 * 7)]
+        "device", "num_ctas", "exchange_copies", "ring_slots", "poll_warps", "engine")] + [("reserved", C.c_int32 * 6)]
 
 
 class wn_layer_weights(C.Structure):
@@ -72,7 +72,7 @@ class wn_stream_open_args(C.Structure):
     _fields_ = [("B", C.c_int32), ("g", C.c_void_p), ("initial", C.c_void_p), ("initial_index", C.c_int32),
                 ("initial_rows", C.c_void_p), ("initial_dense", C.c_void_p), ("flags", C.c_uint32),
                 ("noise_kind", C.c_int32), ("seed", C.c_uint64), ("philox_row0", C.c_int32), ("stream", C.c_void_p),
-                ("reserved", C.c_int32 * 6)]
+                ("engine", C.c_int32), ("reserved", C.c_int32 * 5)]
 
 
 class wn_stream_chunk(C.Structure):

@@ -75,7 +75,19 @@ struct Wn7Ptrs {
     long long* prof;           // optional [P][16] cycle counters
     int warp_reverse;          // 1: logical warp = (warps-1) - physical warp
     int defer_gate;            // 1: deferred passes start only after every compute warp has published its critical rows
+    // ---- streaming (wn_stream_generate, wn7_stream_kernel): a launch continues an utterance at absolute step t_base
+    unsigned t_base;           // absolute step of local step 0 (Philox counters, ring positions)
+    float* state;              // [P][ring floats] rings then the feedback [BT] s_in, [BT] s_idx, [BT][O] s_dense
+    int state_load;            // 1: rings and step-0 feedback come from `state`; 0: zero rings, feedback from initial*
 };
+
+// floats of a stream's state: the history rings of one block, then (once) the feedback of the next step
+__host__ __device__ inline long long wn7_state_ring_floats(const Wn7Plan& pl) {
+    return pl.ring_pos_total * 4 * pl.qA * pl.BT;
+}
+__host__ __device__ inline long long wn7_state_feedback_floats(const Wn7Plan& pl) {
+    return 2LL * pl.BT + (pl.input_kind != 0 ? (long long)pl.BT * pl.O : 0);
+}
 
 #define WN7_FLAG_SOFTMAX 1u
 #define WN7_FLAG_QUANTIZE 2u
@@ -199,7 +211,9 @@ __device__ __forceinline__ void reduce32(float (&v)[NV], int lane) {
 
 // SELF: no dedicated polling warps -- compute warps 0..WN7_NSP-1 poll the vector themselves (their share each), meet
 // at a named barrier and go straight into their passes; the other compute warps are released through the mbarrier.
-template <int BT, bool SELF>
+// STREAM: the kernel of wn_stream_generate (absolute steps, history and feedback in a state buffer); a separate
+// __global__ (wn7_stream_kernel), so the whole-utterance kernels compile exactly as without it.
+template <int BT, bool SELF, bool STREAM = false>
 struct Engine {
     static constexpr int NV = 2 * BT;          // values of one pass: 2 rows x BT utterances, index r*BT + b
     const Wn7Plan& pl;
@@ -466,6 +480,7 @@ struct Engine {
         float* nz = noise_() + (size_t)b * (pl.O + 2);
         const int B = pp.Btot, K = pl.Kmix, O = pl.O;
         const uint32_t ub = (uint32_t)(pp.b0 + b);
+        const uint32_t tc = (STREAM ? pp.t_base : 0u) + (uint32_t)t;   // Philox counts absolute steps; replay is per launch
         const bool replay = pp.noise_kind == 0;
         const uint2 key = make_uint2((uint32_t)pp.seed, (uint32_t)(pp.seed >> 32));
         if (b >= pp.B) {   // padding row of the batch tile: harmless constants
@@ -477,7 +492,7 @@ struct Engine {
                 float e;
                 if (replay) e = pp.e ? __ldg(pp.e + ((size_t)t * B + b) * O + i) : 1.0f;
                 else {
-                    const uint4 r = philox4(make_uint4((uint32_t)t, ub, (uint32_t)i, 2u), key);
+                    const uint4 r = philox4(make_uint4(tc, ub, (uint32_t)i, 2u), key);
                     e = -logf(u01(r.x));
                 }
                 nz[i] = e;
@@ -489,7 +504,7 @@ struct Engine {
             for (int i = lane; i < K; i += 32) {
                 float u;
                 if (replay) u = __ldg(pp.u1 + ((size_t)t * B + b) * K + i);
-                else u = u01(philox4(make_uint4((uint32_t)t, ub, (uint32_t)i, 0u), key).x);
+                else u = u01(philox4(make_uint4(tc, ub, (uint32_t)i, 0u), key).x);
                 nz[i] = u;
             }
         }
@@ -497,11 +512,11 @@ struct Engine {
             float v;
             if (pl.head_kind == 0) {
                 if (replay) v = __ldg(pp.u2 + (size_t)t * B + b);
-                else v = u01(philox4(make_uint4((uint32_t)t, ub, 0u, 1u), key).x);
+                else v = u01(philox4(make_uint4(tc, ub, 0u, 1u), key).x);
             } else {
                 if (replay) v = __ldg(pp.z + (size_t)t * B + b);
                 else {
-                    const uint4 r = philox4(make_uint4((uint32_t)t, ub, 0u, 1u), key);
+                    const uint4 r = philox4(make_uint4(tc, ub, 0u, 1u), key);
                     v = sqrtf(-2.f * logf(u01(r.x))) * cospif(2.f * u01(r.y));   // Box-Muller
                 }
             }
@@ -1085,122 +1100,46 @@ struct Engine {
 // ------------------------------------------------------------------------------------------
 // kernel entry
 // ------------------------------------------------------------------------------------------
+// Stream epilogue (every thread, after the block barrier that follows the role loops): the rings in shared memory and
+// block 0's feedback of the step after the launch.  Nothing else carries over a step: the stage buffers xin / xown /
+// x0own / hs / noise are filled before they are read within the step, skipacc restarts at layer 1, the pre-sum table
+// and the conditioning double buffer are rebuilt per step by HK and COND, and the exchange tags count local steps.
+template <int BT>
+__device__ __noinline__ void wn7_store_state(const Wn7Plan& pl, const Wn7Ptrs& pp, unsigned char* sm) {
+    const int tid = (int)threadIdx.x, NT = (int)blockDim.x, p = (int)blockIdx.x;
+    const long long ring_n = wn7_state_ring_floats(pl);
+    if (pl.ring_in_smem) {
+        const volatile float* ring = reinterpret_cast<const volatile float*>(sm + pl.sm_ring);
+        float* dst = pp.state + (size_t)p * ring_n;
+        for (long long i = tid; i < ring_n; i += NT) dst[i] = ring[i];
+    }
+    if (p == 0) {
+        const float* s_in = reinterpret_cast<const float*>(sm + pl.sm_in);      // layout of Engine's s_in_ / s_idx_ / s_dense_
+        const int* s_idx = reinterpret_cast<const int*>(s_in + BT);
+        const float* s_dense = reinterpret_cast<const float*>(s_idx + BT);
+        float* fb = pp.state + (size_t)pl.P * ring_n;
+        for (int b = tid; b < BT; b += NT) {
+            fb[b] = s_in[b];
+            fb[BT + b] = __int_as_float(s_idx[b]);
+        }
+        if (pl.input_kind != 0)
+            for (int i = tid; i < BT * pl.O; i += NT) fb[2 * BT + i] = s_dense[i];
+    }
+}
+
 template <int BT, bool SELF>
 __global__ void __launch_bounds__(32 * ((SELF ? 0 : WN7_MAX_NPW) + WN7_NCW + 3), 1)
 wn7_kernel(const __grid_constant__ Wn7Plan pl, const __grid_constant__ Wn7Ptrs pp) {
-    extern __shared__ __align__(1024) unsigned char smem_raw[];
-    Engine<BT, SELF> eng(pl, pp, smem_raw);
-    const int npollw = SELF ? WN7_NSP : pl.npw;
-    const int tid = eng.tid, p = blockIdx.x, warp = eng.warp, NT = pl.nthreads;     // logical indices (see Engine)
-    const int nslots = pl.nres + pl.nring;
-    const int L = pl.L, RA4 = 4 * pl.qA;
-    if (tid == 0) {
-        for (int i = 0; i < nslots; ++i) mbar_init(&eng.bar_full_()[i], 1);
-        for (int i = 0; i < pl.nring; ++i) mbar_init(&eng.bar_empty_()[i], WN7_NCW);
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&eng.bar_cfull_()[i], 1);
-            mbar_init(&eng.bar_cempty_()[i], 1);
-            mbar_init(&eng.bar_in_()[i], npollw);
-            mbar_init(&eng.bar_free_()[i], WN7_NCW);
-        }
-        mbar_init(eng.bar_pre_(), 1);
-        mbar_init(eng.bar_x0_(), npollw);
-        mbar_init(eng.bar_ps_(), npollw);
-        mbar_init(eng.bar_dstep_(), WN7_NCW);
-        mbar_init(&eng.bar_crit_()[0], WN7_NCW);
-        mbar_init(&eng.bar_crit_()[1], WN7_NCW);
-        *eng.s_abort_() = 0;
-        *eng.s_skipcnt_() = 0;
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    // pass table
-    {
-        const int nw = pl.npass * (int)(sizeof(Wn7Pass) / 4);
-        const int* src = reinterpret_cast<const int*>(pp.passes);
-        int* dst = reinterpret_cast<int*>(eng.passes_());
-        for (int i = tid; i < nw; i += NT) dst[i] = src[i];
-    }
-    // zero the history (== the reference's zero-initialised queue, conv.py:35-36) and the scratch buffers
-    if (pl.ring_in_smem) {
-        const size_t n = (size_t)pl.ring_pos_total * RA4 * BT;
-        for (size_t i = tid; i < n; i += NT) eng.ring_()[i] = 0.f;
-    }
-    for (int i = tid; i < 2 * pl.xin_vals * BT; i += NT) eng.xin_()[i] = 0.f;
-    for (int i = tid; i < pl.ms * BT; i += NT) eng.skipacc_()[i] = 0.f;
-    for (int i = tid; i < 2 * pl.mx * BT; i += NT) eng.xown_()[i] = 0.f;
-    for (int i = tid; i < pl.O * BT + 2; i += NT) eng.hs_()[i] = 0.f;
-    for (int i = tid; i < pl.L * (pl.kw - 1); i += NT) {
-        eng.ringtab_()[i * 3] = pp.ringtab[i * 2];           // offset of the ring (in positions)
-        eng.ringtab_()[i * 3 + 1] = pp.ringtab[i * 2 + 1];   // delay D
-        eng.ringtab_()[i * 3 + 2] = 0;                       // t mod D
-    }
-    // biases of the rows this block owns
-    {
-        const float* src = pp.bpack + (size_t)p * pl.cta_b_floats;
-        for (int i = tid; i < pl.cta_b_floats; i += NT) eng.bias_()[i] = src[i];
-    }
-    // first 1x1 conv: [w (scalar input) | b]
-    for (int k = tid; k < pl.R; k += NT) {
-        eng.x0w_()[k] = (pl.input_kind == 0) ? pp.first_w[k] : 0.f;
-        eng.x0w_()[pl.R + k] = pp.first_b[k];
-    }
-    {
-        // static part of the pre-activation: (folded) conv bias + global-conditioning projection
-        // (modules.py:148-152 recomputes Wg.g every step although g is constant; fold it once)
-        const float* bsrc = pp.bpack + (size_t)p * pl.cta_b_floats + pl.bo_zb;
-        const int n = L * RA4 * BT;
-        for (int i = tid; i < n; i += NT) {
-            const int b = i % BT, rr = (i / BT) % RA4, l = i / (BT * RA4);
-            float v = 0.f;
-            if ((rr >> 1) < eng.ny) {
-                v = bsrc[l * 2 * pl.my + rr];
-                if (pp.gbias != nullptr && b < pp.B) {
-                    const int grow = (rr & 1) ? pl.G2 + eng.y0 + (rr >> 1) : eng.y0 + (rr >> 1);
-                    v += pp.gbias[((size_t)b * L + l) * pl.G + grow];
-                }
-            }
-            eng.sb_()[i] = v;
-        }
-    }
-    // feedback for step 0 (wavenet.py:281-301)
-    if (tid < BT) {
-        const int b = tid;
-        float v = 0.f;
-        int idx = -1;
-        if (b < pp.B) {
-            if (pl.input_kind == 0) {
-                if (pp.T_test > 0) v = pp.test_scalar[(size_t)b * pp.T_test];
-                else if (pp.initial) v = pp.initial[b];
-            } else {
-                if (pp.T_test > 0) idx = pp.test_index ? pp.test_index[(size_t)b * pp.T_test] : -1;
-                else if (pp.initial_dense) idx = -1;
-                else if (pp.initial_rows) idx = pp.initial_rows[b];
-                else idx = pp.initial_index;
-            }
-        } else if (pl.input_kind != 0) idx = 0;
-        eng.s_in_()[b] = v;
-        eng.s_idx_()[b] = idx;
-    }
-    if (pl.input_kind != 0) {
-        const float* dsrc = nullptr;
-        size_t stride = 0;
-        if (pp.T_test > 0 && pp.test_dense != nullptr) { dsrc = pp.test_dense; stride = (size_t)pp.T_test * pl.O; }
-        else if (pp.T_test == 0 && pp.initial_dense != nullptr) { dsrc = pp.initial_dense; stride = (size_t)pl.O; }
-        for (int i = tid; i < BT * pl.O; i += NT) {
-            const int b = i / pl.O, o = i % pl.O;
-            eng.s_dense_()[i] = (dsrc && b < pp.B) ? dsrc[(size_t)b * stride + o] : 0.f;
-        }
-    }
-    if (warp < npollw) {
-        for (int b = warp; b < BT; b += npollw) eng.fetch_noise(0, b);
-    }
-    __syncthreads();
+    constexpr bool STREAM = false;
+#include "wn7_kernel_body.cuh"
+}
 
-    if (warp < pl.npw) eng.poll_loop();
-    else if (warp < wn7_warp_hk(pl)) eng.comp_loop();
-    else if (warp == wn7_warp_hk(pl)) eng.hk_loop();
-    else if (warp == wn7_warp_tma(pl)) eng.tma_loop();
-    else if (pl.C > 0) eng.cond_loop();
+// wn_stream_generate's kernel: handles whose compute warps poll (SELF), BT = 1, 2, 4, 8
+template <int BT>
+__global__ void __launch_bounds__(32 * (WN7_NCW + 3), 1)
+wn7_stream_kernel(const __grid_constant__ Wn7Plan pl, const __grid_constant__ Wn7Ptrs pp) {
+    constexpr bool SELF = true, STREAM = true;
+#include "wn7_kernel_body.cuh"
 }
 
 }  // namespace wn7

@@ -440,7 +440,13 @@ static int32_t check_weights(const wn_config& c, const wn_weights* w) {
 // alternative: row-pair passes finalised inside the warp, up to 8 utterances per launch (csrc/wn7_kernel.cuh).
 // Both are parity-tested.  On an H100 SXM (700 W) 7 is 20 % slower at B = 1 (config 2) and 46 % faster for 8
 // utterances (config 4), which it runs in one launch (DESIGN.md 7).
-static int engine_choice() { return env_int("WN_ENGINE", 5) == 7 ? 7 : 5; }
+// wn_config.engine: 0 = WN_ENGINE (7, else 5); 5 or 7 = that engine, whatever WN_ENGINE says.
+static int32_t engine_choice(const wn_config& c, int* engine) {
+    if (c.engine == 0) *engine = env_int("WN_ENGINE", 5) == 7 ? 7 : 5;
+    else if (c.engine == 5 || c.engine == 7) *engine = c.engine;
+    else return fail(WN_ERR_INVALID, "wn_config.engine must be 0 (WN_ENGINE, else 5), 5 or 7; got " + std::to_string(c.engine));
+    return WN_OK;
+}
 
 // ------------------------------------------------------------------------------------------
 // handle
@@ -452,7 +458,7 @@ struct WnHandle {
     std::vector<Wn7Pass> passes7;
     float* d_bpack = nullptr;
     Wn7Pass* d_passes = nullptr;
-    bool attr7_set[8] = {};
+    bool attr7_set[12] = {};      // [0, 8): whole utterances (BT x polling warps or not), [8, 12): the stream kernels
     // local-conditioning upsampler (wn_load_upsampler)
     bool have_ups = false;
     wnaux::UpsampleDesc ups;
@@ -762,7 +768,15 @@ static int32_t run_upsampler(WnHandle* h, const float* c_frames, int B, int F, i
     return WN_OK;
 }
 
-static const void* kernel7_for(int BT, bool self) {
+static const void* kernel7_for(int BT, bool self, bool stream) {
+    if (stream) {       // wn7_kernel.cuh: streams run on handles whose compute warps poll
+        switch (BT) {
+            case 1: return (const void*)wn7::wn7_stream_kernel<1>;
+            case 2: return (const void*)wn7::wn7_stream_kernel<2>;
+            case 4: return (const void*)wn7::wn7_stream_kernel<4>;
+            default: return (const void*)wn7::wn7_stream_kernel<8>;
+        }
+    }
     if (self) {
         switch (BT) {
             case 1: return (const void*)wn7::wn7_kernel<1, true>;
@@ -779,16 +793,17 @@ static const void* kernel7_for(int BT, bool self) {
     }
 }
 
-static int32_t prepare_kernel7(WnHandle* h, int BT, bool self) {
-    const int ai = bt_index(BT) + (self ? 4 : 0);
+static int32_t prepare_kernel7(WnHandle* h, int BT, bool self, bool stream) {
+    const int ai = bt_index(BT) + (stream ? 8 : (self ? 4 : 0));
     if (h->attr7_set[ai]) return WN_OK;
-    const void* fn = kernel7_for(BT, self);
+    const void* fn = kernel7_for(BT, self, stream);
     CUDA_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_cap));
     h->attr7_set[ai] = true;
     return WN_OK;
 }
 
-static int32_t launch_chunk7(WnHandle* h, const wn_generate_args* a, int b0, int Bc, cudaStream_t st) {
+static int32_t launch_chunk7(WnHandle* h, const wn_generate_args* a, int b0, int Bc, cudaStream_t st,
+                             const StreamCtx* sc = nullptr) {
     Wn7Plan pl;
     std::vector<Wn7Pass> passes;
     std::vector<int> rt;
@@ -802,7 +817,8 @@ static int32_t launch_chunk7(WnHandle* h, const wn_generate_args* a, int b0, int
     rc = ensure(&h->d_xbuf, &h->xbuf_bytes, xb);
     if (rc) return rc;
     CUDA_TRY(cudaMemsetAsync(h->d_xbuf, 0, xb, st));     // zeroed every call so stale tags can never match
-    if (!pl.ring_in_smem) {
+    if (sc && pl.npw != 0) return fail(WN_ERR_INVALID, "an engine-7 stream needs a handle whose compute warps poll");
+    if (!pl.ring_in_smem && !sc) {         // a stream's global-memory rings are its state buffer (zeroed at open)
         const size_t rb = std::max<size_t>(16, (size_t)pl.P * pl.ring_pos_total * 4 * pl.qA * BT * sizeof(float));
         rc = ensure(&h->d_ring, &h->ring_bytes, rb);
         if (rc) return rc;
@@ -810,7 +826,12 @@ static int32_t launch_chunk7(WnHandle* h, const wn_generate_args* a, int b0, int
     }
     Wn7Ptrs pp;
     memset(&pp, 0, sizeof(pp));
-    if (c.gin_channels > 0) {
+    if (sc) {
+        pp.state = sc->state;
+        pp.state_load = sc->state_load;
+        pp.t_base = sc->t_base;
+        pp.gbias = sc->gbias;
+    } else if (c.gin_channels > 0) {
         if (!a->g) return fail(WN_ERR_INVALID, "g is required (gin_channels > 0), cf. train.py:72-80 sanity_check");
         const size_t gb = (size_t)Bc * pl.L * pl.G * sizeof(float);
         rc = ensure(&h->d_gbias, &h->gbias_bytes, gb);
@@ -830,7 +851,7 @@ static int32_t launch_chunk7(WnHandle* h, const wn_generate_args* a, int b0, int
     pp.first_w = h->d_first_w;
     pp.first_b = h->d_first_b;
     pp.xbuf = h->d_xbuf;
-    pp.ring_g = h->d_ring;
+    pp.ring_g = (sc && !pl.ring_in_smem) ? sc->state : h->d_ring;
     pp.ringtab = h->d_ringtab;
     pp.err = h->d_err;
     set_call_args(pp, a, b0, Bc, pl.C, pl.O, pl.Kmix);
@@ -842,7 +863,7 @@ static int32_t launch_chunk7(WnHandle* h, const wn_generate_args* a, int b0, int
         CUDA_TRY(cudaMemsetAsync(h->d_prof, 0, pb, st));
         pp.prof = h->d_prof;
     }
-    rc = prepare_kernel7(h, BT, pl.npw == 0);
+    rc = prepare_kernel7(h, BT, pl.npw == 0, sc != nullptr);
     if (rc) return rc;
     void* kargs[2] = {(void*)&pl, (void*)&pp};
     // cooperative launch: the runtime refuses to start unless all P blocks are co-resident, which the
@@ -869,7 +890,7 @@ static int32_t launch_chunk7(WnHandle* h, const wn_generate_args* a, int b0, int
     }
     lc.attrs = la;
     lc.numAttrs = na;
-    CUDA_TRY(cudaLaunchKernelExC(&lc, kernel7_for(BT, pl.npw == 0), kargs));
+    CUDA_TRY(cudaLaunchKernelExC(&lc, kernel7_for(BT, pl.npw == 0, sc != nullptr), kargs));
     h->launches++;
     return WN_OK;
 }
@@ -989,7 +1010,9 @@ const char* wn_last_error(void) { return g_err.c_str(); }
 
 int32_t wn_plan_only(const wn_config* cfg, int32_t batch, int32_t num_sms, int64_t smem_per_cta, wn_plan_info* out) {
     if (!cfg || !out) return fail(WN_ERR_INVALID, "null argument");
-    if (engine_choice() == 7) {
+    int engine = 5;
+    if (int32_t rce = engine_choice(*cfg, &engine)) return rce;
+    if (engine == 7) {
         Wn7Plan pl6;
         std::vector<Wn7Pass> ps;
         std::vector<int> rt6;
@@ -1009,6 +1032,8 @@ int32_t wn_plan_only(const wn_config* cfg, int32_t batch, int32_t num_sms, int64
 int32_t wn_plan_passes(const wn_config* cfg, int32_t batch, int32_t num_sms, int64_t smem_per_cta, int32_t* plan_words,
                        int32_t max_plan_words, void* passes, int32_t max_passes) {
     if (!cfg) return fail(WN_ERR_INVALID, "null argument");
+    int engine = 5;            // the pass table is engine 7's whichever engine the config picks; a bad value is refused
+    if (int32_t rce = engine_choice(*cfg, &engine)) return rce;
     Wn7Plan pl;
     std::vector<Wn7Pass> ps;
     std::vector<int> rt;
@@ -1028,7 +1053,9 @@ int32_t wn_plan_passes(const wn_config* cfg, int32_t batch, int32_t num_sms, int
 int32_t wn_pack_cta(const wn_config* cfg, int32_t batch, int32_t num_sms, int64_t smem_per_cta, const wn_weights* w,
                     int32_t cta, float* packed, int64_t packed_floats) {
     if (!cfg || !packed) return fail(WN_ERR_INVALID, "null argument");
-    if (engine_choice() == 7) {
+    int engine = 5;
+    if (int32_t rce = engine_choice(*cfg, &engine)) return rce;
+    if (engine == 7) {
         Wn7Plan pl6;
         std::vector<Wn7Pass> ps;
         std::vector<int> rt6;
@@ -1082,9 +1109,11 @@ int32_t wn_create(const wn_config* cfg, void** handle) {
     int coop = 0;
     CUDA_TRY(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, cfg->device));
     if (!coop) return fail(WN_ERR_CUDA, "device does not support cooperative launch");
+    int engine = 5;
+    if (int32_t rce = engine_choice(*cfg, &engine)) return rce;
     WnHandle* h = new WnHandle();
     h->cfg = *cfg;
-    h->engine = engine_choice();
+    h->engine = engine;
     h->num_sms = prop.multiProcessorCount;
     h->smem_cap = (long long)prop.sharedMemPerBlockOptin;
     h->l2_bytes = (size_t)prop.l2CacheSize;
@@ -1578,9 +1607,10 @@ int32_t wn_decode(const float* y_scalar, const int32_t* y_index, int32_t B, int3
 struct WnStream {
     WnHandle* h = nullptr;
     int B = 0;
+    int engine = 5;                // the kernel organisation the chunks run on (wn_stream_open_args.engine)
     uint64_t weight_gen = 0;       // the handle's weights this stream was opened with
     wn_stream_open_args open;      // initial* point into d_init (copies made at open)
-    float* d_state = nullptr;      // P x rings, then the feedback (wn_kernel.cuh WnPtrs::state)
+    float* d_state = nullptr;      // P x rings, then the feedback (WnPtrs::state / Wn7Ptrs::state)
     float* d_gbias = nullptr;
     float* d_init = nullptr;
     long long t = 0;               // absolute step of the next sample
@@ -1592,23 +1622,57 @@ int32_t wn_stream_open(void* handle, const wn_stream_open_args* a, void** stream
     if (!h || !a || !stream) return fail(WN_ERR_INVALID, "null argument");
     *stream = nullptr;
     if (!h->have_weights) return fail(WN_ERR_STATE, "wn_stream_open before wn_load_weights");
-    if (h->engine != 5) return fail(WN_ERR_INVALID, "streaming runs on engine 5 only (WN_ENGINE=7 was chosen)");
-    const int tile = std::min(4, max_tile(5));
-    if (a->B < 1 || a->B > tile)
-        return fail(WN_ERR_INVALID, "a stream holds 1.." + std::to_string(tile) + " utterances (one batch tile)");
+    if (a->engine != 0 && a->engine != 5 && a->engine != 7)
+        return fail(WN_ERR_INVALID, "wn_stream_open_args.engine must be 0 or 5 (engine 5) or 7; got " + std::to_string(a->engine));
+    const int engine = a->engine == 7 ? 7 : 5;
+    if (engine == 5) {
+        if (h->engine != 5)
+            return fail(WN_ERR_INVALID, "this stream runs on engine 5 but the handle runs engine 7 (WN_ENGINE=7 or "
+                                        "wn_config.engine = 7): open it with wn_stream_open_args.engine = 7");
+        const int tile = std::min(4, max_tile(5));
+        if (a->B < 1 || a->B > tile)
+            return fail(WN_ERR_INVALID, "a stream holds 1.." + std::to_string(tile) + " utterances (one batch tile)");
+    } else {
+        if (h->engine != 7)
+            return fail(WN_ERR_INVALID, "an engine-7 stream needs a handle that runs engine 7 (wn_config.engine = 7); "
+                                        "this one runs engine 5");
+        if (h->base7.npw != 0)
+            return fail(WN_ERR_INVALID, "an engine-7 stream needs a handle whose compute warps poll (poll_warps 0 or -1); "
+                                        "this one has " + std::to_string(h->base7.npw) + " polling warps");
+        const int tile = max_tile(7);
+        if (a->B < 1 || a->B > tile)
+            return fail(WN_ERR_INVALID, "an engine-7 stream holds 1.." + std::to_string(tile) +
+                                            " utterances (one batch tile)");
+    }
     const wn_config& c = h->cfg;
     if (c.gin_channels > 0 && !a->g) return fail(WN_ERR_INVALID, "g is required (gin_channels > 0), cf. train.py:72-80 sanity_check");
     if (c.gin_channels == 0 && a->g) return fail(WN_ERR_INVALID, "g given but the model has no global conditioning");
     if (a->noise_kind != WN_NOISE_REPLAY && a->noise_kind != WN_NOISE_PHILOX) return fail(WN_ERR_INVALID, "bad noise_kind");
     DeviceGuard guard(c.device);
-    WnPlan pl;
-    std::vector<int> rt;
-    int32_t rc = build_plan(c, a->B, h->num_sms, h->smem_cap, pl, rt);
-    if (rc) return rc;
+    // the state buffer: every block's history rings, then the feedback of the next step
+    size_t state_floats = 0;
+    int L = 0, G = 0, O = 0;
+    if (engine == 5) {
+        WnPlan pl;
+        std::vector<int> rt;
+        int32_t rc = build_plan(c, a->B, h->num_sms, h->smem_cap, pl, rt);
+        if (rc) return rc;
+        state_floats = (size_t)pl.P * wn_state_ring_floats(pl) + wn_state_feedback_floats(pl);
+        L = pl.L, G = pl.G, O = pl.O;
+    } else {
+        Wn7Plan pl;
+        std::vector<Wn7Pass> ps;
+        std::vector<int> rt;
+        int32_t rc = build_plan7(c, a->B, h->num_sms, h->smem_cap, pl, ps, rt);
+        if (rc) return rc;
+        state_floats = (size_t)pl.P * wn7_state_ring_floats(pl) + wn7_state_feedback_floats(pl);
+        L = pl.L, G = pl.G, O = pl.O;
+    }
     cudaStream_t st = (cudaStream_t)a->stream;
     WnStream* s = new WnStream();
     s->h = h;
     s->B = a->B;
+    s->engine = engine;
     s->weight_gen = h->weight_gen;
     s->open = *a;
     auto bail = [&](int32_t code) {
@@ -1616,9 +1680,8 @@ int32_t wn_stream_open(void* handle, const wn_stream_open_args* a, void** stream
         delete s;
         return code;
     };
-    const size_t state_floats = (size_t)pl.P * wn_state_ring_floats(pl) + wn_state_feedback_floats(pl);
     if (cudaMalloc((void**)&s->d_state, state_floats * sizeof(float)) != cudaSuccess ||
-        cudaMalloc((void**)&s->d_init, ((size_t)2 + pl.O) * a->B * sizeof(float)) != cudaSuccess)
+        cudaMalloc((void**)&s->d_init, ((size_t)2 + O) * a->B * sizeof(float)) != cudaSuccess)
         return bail(fail(WN_ERR_NOMEM, "cudaMalloc of the stream state failed"));
     if (cudaMemsetAsync(s->d_state, 0, state_floats * sizeof(float), st) != cudaSuccess)
         return bail(fail(WN_ERR_CUDA, "cudaMemsetAsync of the stream state failed"));
@@ -1631,7 +1694,7 @@ int32_t wn_stream_open(void* handle, const wn_stream_open_args* a, void** stream
     };
     if ((a->initial && !copy(init, a->initial, a->B * sizeof(float))) ||
         (a->initial_rows && !copy(init_rows, a->initial_rows, a->B * sizeof(int32_t))) ||
-        (a->initial_dense && !copy(init_dense, a->initial_dense, (size_t)a->B * pl.O * sizeof(float))))
+        (a->initial_dense && !copy(init_dense, a->initial_dense, (size_t)a->B * O * sizeof(float))))
         return bail(fail(WN_ERR_CUDA, "copying the initial input failed"));
     s->open.initial = a->initial ? init : nullptr;
     s->open.initial_rows = a->initial_rows ? init_rows : nullptr;
@@ -1639,9 +1702,9 @@ int32_t wn_stream_open(void* handle, const wn_stream_open_args* a, void** stream
     s->open.g = nullptr;
     if (c.gin_channels > 0) {
         // Wg . g once per stream (modules.py:148-152 recomputes it every step although g is constant)
-        if (cudaMalloc((void**)&s->d_gbias, (size_t)a->B * pl.L * pl.G * sizeof(float)) != cudaSuccess)
+        if (cudaMalloc((void**)&s->d_gbias, (size_t)a->B * L * G * sizeof(float)) != cudaSuccess)
             return bail(fail(WN_ERR_NOMEM, "cudaMalloc of the stream's global-conditioning bias failed"));
-        wn::wn_gbias_kernel<<<dim3(pl.L, a->B), 128, 0, st>>>(h->d_wg, a->g, s->d_gbias, pl.L, pl.G, c.gin_channels);
+        wn::wn_gbias_kernel<<<dim3(L, a->B), 128, 0, st>>>(h->d_wg, a->g, s->d_gbias, L, G, c.gin_channels);
         h->launches++;
     }
     if (cudaStreamSynchronize(st) != cudaSuccess || cudaGetLastError() != cudaSuccess)
@@ -1708,7 +1771,7 @@ int32_t wn_stream_generate(void* stream, const wn_generate_args* chunk, const wn
     sc.state_load = s->t > 0 ? 1 : 0;
     sc.t_base = (unsigned)s->t;
     sc.gbias = s->d_gbias;
-    rc = launch_chunk(h, &a, 0, a.B, st, &sc);
+    rc = s->engine == 7 ? launch_chunk7(h, &a, 0, a.B, st, &sc) : launch_chunk(h, &a, 0, a.B, st, &sc);
     if (rc) return rc;
     s->t += a.T;
     if (where && where->final) s->final = true;

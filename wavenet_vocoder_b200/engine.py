@@ -74,9 +74,10 @@ def weights_struct(sd: Dict[str, torch.Tensor], layers: int, cin: int, gin: int)
 
 def make_config(*, layers, stacks, residual_channels, gate_channels, skip_out_channels, out_channels,
                 kernel_size, cin_channels, gin_channels, scalar_input, output_distribution,
-                device_index=0, num_ctas=0, exchange_copies=0, ring_slots=0, poll_warps=0):
+                device_index=0, num_ctas=0, exchange_copies=0, ring_slots=0, poll_warps=0, engine=0):
     """wn_config from the reference's constructor keywords (wavenet.py:98-111).  num_ctas, exchange_copies,
-    ring_slots and poll_warps are the planner's fields of include/wn.h (0 = the planner chooses)."""
+    ring_slots and poll_warps are the planner's fields of include/wn.h (0 = the planner chooses); engine is the kernel
+    organisation (0 = WN_ENGINE, else 5; 5 or 7 = that one)."""
     if scalar_input:
         if output_distribution == "Logistic":
             head = N.WN_HEAD_MOL
@@ -98,6 +99,7 @@ def make_config(*, layers, stacks, residual_channels, gate_channels, skip_out_ch
     cfg.device = int(device_index)
     cfg.num_ctas = int(num_ctas)
     cfg.exchange_copies, cfg.ring_slots, cfg.poll_warps = int(exchange_copies), int(ring_slots), int(poll_warps)
+    cfg.engine = int(engine)
     return cfg
 
 
@@ -188,14 +190,17 @@ def nll(head: torch.Tensor, head_kind: int, target: torch.Tensor, num_classes: i
 
 class SynthesisStream:
     """One utterance (or one batch tile of them) made chunk by chunk; the state between chunks stays on the device
-    (wn_stream_* of include/wn.h).  Chunks are bit-identical to the same samples of one ``generate`` call."""
+    (wn_stream_* of include/wn.h).  Chunks are bit-identical to the same samples of one ``generate`` call on the same
+    handle.  ``engine``: 0 or 5 = an engine-5 stream (1..4 utterances), 7 = an engine-7 stream (1..8 utterances) on a
+    handle that runs engine 7."""
 
     def __init__(self, eng, *, B, g=None, initial=None, initial_index=-1, initial_rows=None, initial_dense=None,
-                 softmax=True, quantize=True, replay=False, seed=None, philox_row0=0):
+                 softmax=True, quantize=True, replay=False, seed=None, philox_row0=0, engine=0):
         self.eng, self.B, self.quantize = eng, int(B), bool(quantize)
         dev = eng.device
         a = N.wn_stream_open_args()
         a.B = self.B
+        a.engine = int(engine)
         hold = []
 
         def dptr(t, dtype=torch.float32, shape=None):
@@ -308,7 +313,7 @@ class SynthesisEngine:
     def __init__(self, *, layers, stacks, residual_channels, gate_channels, skip_out_channels,
                  out_channels, kernel_size, cin_channels, gin_channels, scalar_input,
                  output_distribution, device: torch.device, num_ctas=0, exchange_copies=0, ring_slots=0,
-                 poll_warps=0):
+                 poll_warps=0, engine=0):
         if device.type != "cuda":
             raise RuntimeError("wavenet_vocoder_b200 runs the synthesis path on a CUDA device only "
                                "(there is no CPU fallback); got device %s" % device)
@@ -324,7 +329,7 @@ class SynthesisEngine:
                           output_distribution=output_distribution,
                           device_index=device.index if device.index is not None else torch.cuda.current_device(),
                           num_ctas=num_ctas, exchange_copies=exchange_copies, ring_slots=ring_slots,
-                          poll_warps=poll_warps)
+                          poll_warps=poll_warps, engine=engine)
         self.head = head = cfg.head_kind
         self.K = 0 if head == N.WN_HEAD_SOFTMAX else (1 if out_channels == 2 else out_channels // 3)
         self.cfg = cfg
@@ -335,9 +340,10 @@ class SynthesisEngine:
                           skip_out_channels=skip_out_channels, out_channels=out_channels, kernel_size=kernel_size,
                           cin_channels=cin_channels, gin_channels=gin_channels, scalar_input=scalar_input,
                           output_distribution=output_distribution, device=device,
-                          exchange_copies=exchange_copies, ring_slots=ring_slots, poll_warps=poll_warps)
+                          exchange_copies=exchange_copies, ring_slots=ring_slots, poll_warps=poll_warps, engine=engine)
         self._sd = None
         self._halves = None           # two half-grid engines for concurrent batch tiles (see generate_concurrent)
+        self._sib7 = None             # an engine-7 engine of the same model for engine-7 streams (see engine7)
         self._is_child = num_ctas > 0
         self._ups = None
         self._streams = weakref.WeakSet()   # open SynthesisStreams: closed before the handle they run on
@@ -348,6 +354,9 @@ class SynthesisEngine:
         for ch in (getattr(self, "_halves", None) or []):
             ch["eng"].close()
         self._halves = None
+        if getattr(self, "_sib7", None) is not None:
+            self._sib7.close()
+        self._sib7 = None
         if getattr(self, "_h", None) is not None and self._h.value:
             N.lib().wn_destroy(self._h)
             self._h = C.c_void_p()
@@ -369,6 +378,9 @@ class SynthesisEngine:
             for ch in (self._halves or []):
                 ch["eng"].close()
             self._halves = None
+            if self._sib7 is not None:
+                # reloaded, not closed: its open streams then refuse their next chunk (the weights changed)
+                self._sib7.load_state_dict(sd)
 
     def load_upsampler(self, net) -> bool:
         """Hand the local-conditioning upsampler (upsample.py:29-85 there) to libwn so that ``generate`` can take
@@ -378,6 +390,8 @@ class SynthesisEngine:
         self._ups_net = net
         for ch in (getattr(self, "_halves", None) or []):
             ch["eng"].load_upsampler(net)
+        if getattr(self, "_sib7", None) is not None:
+            self._sib7.load_upsampler(net)
         self.ups_frames_lost = 0
         self.ups_total = 1
         self._ups = None
@@ -550,8 +564,25 @@ class SynthesisEngine:
 
     # ------------------------------------------------------------------ streaming
     def open_stream(self, **kw) -> SynthesisStream:
-        """A stream of chunks on this handle (keywords of SynthesisStream); one batch tile, engine 5."""
+        """A stream of chunks on this handle (keywords of SynthesisStream); one batch tile.  ``engine=7`` opens an
+        engine-7 stream of up to 8 utterances, which needs a handle created with ``engine=7``."""
         return SynthesisStream(self, **kw)
+
+    def engine7(self) -> "SynthesisEngine":
+        """This engine if it runs engine 7, else an engine-7 engine of the same model on the same device, made on
+        first use with this engine's weights and upsampler, reloaded with them and closed with this engine."""
+        if self.plan(1)["engine"] == 7:
+            return self
+        if self._sib7 is None:
+            if self._sd is None:
+                raise RuntimeError("load_state_dict first")
+            e = SynthesisEngine(**dict(self._ctor, engine=7))
+            e._is_child = True            # its weights are this engine's: nothing to keep twice
+            e.load_state_dict(self._sd)
+            if getattr(self, "_ups_net", None) is not None:
+                e.load_upsampler(self._ups_net)
+            self._sib7 = e
+        return self._sib7
 
     # ------------------------------------------------------------------ two batch tiles at a time
     def generate_concurrent(self, *, B: int, T: int, c: Optional[torch.Tensor] = None,

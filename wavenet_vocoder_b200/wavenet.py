@@ -439,16 +439,21 @@ class WaveNet(nn.Module):
     # ------------------------------------------------------------------ streaming
     @torch.no_grad()
     def open_stream(self, B=1, g=None, initial_input=None, seed=None, noise=None, softmax=True, quantize=True,
-                    return_params=False):
+                    return_params=False, engine=None):
         """Synthesis in chunks: a ``WaveNetStream`` whose chunks concatenate to exactly what ``incremental_forward``
         returns for the whole utterance with the same ``g``, ``initial_input``, ``seed`` or ``noise`` (the whole
         utterance's replayed draws, sliced per chunk) and conditioning.  The state between chunks (history queues,
-        fed-back sample, noise position) stays on the device.  At most one batch tile (4 utterances); no teacher
-        forcing; engine 5."""
+        fed-back sample, noise position) stays on the device.  One batch tile; no teacher forcing.
+
+        ``engine``: None (or 5) streams on the model's engine-5 handle, at most 4 utterances.  7 streams up to 8
+        utterances on engine 7: on the model's own handle if it runs engine 7, else on an engine-7 handle of the same
+        weights made on first use (``SynthesisEngine.engine7``).  Its chunks are bit-identical to one ``generate`` call
+        on an engine-7 handle; for B > 4 they match the default ``incremental_forward`` (engine 5, two tiles) only to
+        fp32 tolerance, because the two engines sum in different orders."""
         if self.training:
             raise RuntimeError("open_stream only supports eval mode")
         return WaveNetStream(self, B=int(B), g=g, initial_input=initial_input, seed=seed, noise=noise,
-                             softmax=softmax, quantize=quantize, return_params=return_params)
+                             softmax=softmax, quantize=quantize, return_params=return_params, engine=engine)
 
 
 class WaveNetStream:
@@ -458,7 +463,7 @@ class WaveNetStream:
     arrive and returns the samples whose frames are all known (possibly none); ``finish()`` returns the rest, up to
     the upsampled length of all frames pushed.  Outputs are laid out as ``incremental_forward``'s."""
 
-    def __init__(self, model, *, B, g, initial_input, seed, noise, softmax, quantize, return_params):
+    def __init__(self, model, *, B, g, initial_input, seed, noise, softmax, quantize, return_params, engine=None):
         self._m = model
         self._eng = eng = model._get_engine()
         dev = eng.device
@@ -489,8 +494,10 @@ class WaveNetStream:
                 else:
                     initial_dense = first
         self._noise = None if noise is None else {k: v.to(dev) for k, v in noise.items()}
-        self._s = eng.open_stream(B=B, g=g_vec, initial=initial, initial_rows=initial_rows, initial_dense=initial_dense,
-                                  softmax=bool(softmax), quantize=bool(quantize), replay=noise is not None, seed=seed)
+        seng = eng.engine7() if engine == 7 else eng          # the handle the chunks run on
+        self._s = seng.open_stream(B=B, g=g_vec, initial=initial, initial_rows=initial_rows, initial_dense=initial_dense,
+                                   softmax=bool(softmax), quantize=bool(quantize), replay=noise is not None, seed=seed,
+                                   engine=0 if engine is None else int(engine))
         self.B, self._quantize, self._return_params = B, bool(quantize), bool(return_params)
         self._frames = None          # every frame pushed so far, (B,C,n) on the device
         self._finished = False
